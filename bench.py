@@ -1,8 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- video-latent tokens/s per denoising step of the Wan DiT forward on B200(s).
+"""bench.py -- video-latent tokens/s per denoising step of the Wan DiT forward on H100(s).
 
   python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torchrun, one rank per GPU)
   python bench.py --impl reference --steps K --warmup W    (the CPU arm: oracle port on the host cores)
+  --dump-outputs DIR: after the timed steps, the output of the last one is written to DIR/model_output.npy (float32; the CPU
+                     arm writes its last timed block's output to DIR/block_output.npy)
 
 Workload (BASELINE.json metric): Wan2.2-T2V-14B architecture (D 5120, 40 heads, ffn 13824, 40 layers), 720p x 81f
 latent 16x21x90x160 -> 75 600 tokens, Video-Sparse attention at sparsity 0.9 (top-k 144 of 1440 tiles), synthetic
@@ -36,25 +38,14 @@ DEFAULT_WORKLOAD = "wan2.2-t2v-14b_720p_81f_vsa0.9"
 METRIC = "video-latent tokens/sec per denoising step"
 
 
-def load_traffic():
-    """Per-launch DRAM bytes of the kernel families from the committed `ncu --set full` capture of this same command
-    (profiles/r2_kernel_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep; dram__bytes_read.sum +
-    dram__bytes_write.sum averaged over the captured launches of the family)."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_kernel_traffic.json")))
-    except Exception:
-        return {}
-
-
-def measured_peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        return None
+# NVIDIA's H100 SXM data sheet (700 W card): dense BF16 tensor rate and HBM3 bandwidth. Shares of peak below are
+# achieved rates over these figures; a card set to a lower power limit reaches less.
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md 'clocks line')."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -104,9 +95,9 @@ CPU_SIZES = (1024, 4096, 9450)  # SURVEY.md section 8d: S in {1024, 4096, 9450} 
 
 
 def _reference_root():
-    """Where the reference's Python lies: the build container has /root/reference; the GPU box only has what
-    oracle/stage_ref_kernels.py staged into oracle/_ref/reference_py (git-ignored, travels with the snapshot)."""
-    for cand in (os.environ.get("FVB_REFERENCE_ROOT"), "/root/reference", os.path.join(ROOT, "oracle", "_ref", "reference_py")):
+    """Where the reference's Python lies: $FVB_REFERENCE_ROOT, else what oracle/stage_ref_kernels.py staged into
+    oracle/_ref/reference_py (git-ignored)."""
+    for cand in (os.environ.get("FVB_REFERENCE_ROOT"), os.path.join(ROOT, "oracle", "_ref", "reference_py")):
         if cand and os.path.isdir(os.path.join(cand, "fastvideo", "models", "dits")):
             return cand
     return None
@@ -183,10 +174,12 @@ class CpuBlock:
             t0 = time.perf_counter()
             if self.blk is not None:
                 with self.ctxmgr(current_timestep=0, attn_metadata=None):
-                    self.blk(x, ctx, temb6, (cos, sin), S)
+                    out = self.blk(x, ctx, temb6, (cos, sin), S)
             else:
-                wan_ref.wan_block(x, ctx, temb6, self.sd, "", H, cos, sin)
-            return time.perf_counter() - t0
+                out = wan_ref.wan_block(x, ctx, temb6, self.sd, "", H, cos, sin)
+            dt = time.perf_counter() - t0
+            self.last_out = out[0] if isinstance(out, (tuple, list)) else out
+            return dt
 
 
 def fit_and_extrapolate(points: dict, S_target: int, layers: int):
@@ -230,7 +223,7 @@ def cpu_arm_measure(arch: dict, S_target: int, steps: int, warmup: int, threads:
               f"extrapolated to S={S_target}: {t_target:.0f} s per block x {arch['num_layers']} layers; dense attention (the "
               f"reference's CPU-runnable path), embedders/head excluded (<1% of FLOPs)")
     return dict(value=value, kind=blk.kind, sample=sample, points=spread, a=a, b=b, t_block_target_s=t_target,
-                step_seconds=step_s)
+                step_seconds=step_s, last_out=blk.last_out)
 
 
 def run_reference_arm(args, rank, world):
@@ -256,7 +249,17 @@ def run_reference_arm(args, rank, world):
             "cpu_baseline": {"value": m["value"], "unit": "tokens/s", "cores": threads, "kind": m["kind"], "sample": m["sample"]},
             "e2e": {"value": m["value"], "unit": "tokens/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": 0}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"block_output": m["last_out"]})
     emit(line)
+
+
+def dump_outputs(directory: str, arrays: dict) -> None:
+    """--dump-outputs: what the timed path returned in its last step, as DIR/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 # HBM-bound row / index kernels of the GPU arm: "work" = algorithmic bytes (every operand row read once, every result row
@@ -344,7 +347,7 @@ def run_gpu_arm(args, rank, world, device):
     arch, latent, text_len, sparsity = WORKLOADS[args.workload]
     arch = dict(arch)
     if args.layers:
-        arch["num_layers"] = args.layers  # development only: flagged in the output, never the driver's run
+        arch["num_layers"] = args.layers  # development only: flagged in the output
     cfg = WanDiTConfig(vsa=sparsity is not None, **arch)
     t0 = time.time()
     model = WanDiT.random(cfg, device)
@@ -364,7 +367,7 @@ def run_gpu_arm(args, rank, world, device):
     vsa_topk = model.layout((T // cfg.patch_size[0], Hh // cfg.patch_size[1], Ww // cfg.patch_size[2]), device, sparsity).topk \
         if sparsity is not None else 0
 
-    # kernel-family timers (dominant kernel = the tcgen05 GEMM; second = the attention kernel)
+    # kernel-family timers (dominant kernel = the wgmma GEMM; second = the attention kernel)
     gemm_t, attn_t, attn_d, rows_t = KernelTimer(), KernelTimer(), KernelTimer(), KernelTimer()
 
     def gemm_work_linear(x, w, *a, **k):
@@ -432,6 +435,8 @@ def run_gpu_arm(args, rank, world, device):
     e1.record()
     sync_all()
     launches = _lib.LAUNCHES - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"model_output": out})
     gemm_t.enabled = attn_t.enabled = attn_d.enabled = rows_t.enabled = False
     ms_total = torch.tensor([e0.elapsed_time(e1)], device=device)
     if world > 1:
@@ -480,25 +485,21 @@ def run_gpu_arm(args, rank, world, device):
 
     if rank != 0:
         return
-    peaks = measured_peaks()
-    peak_tf = (peaks or {}).get("bf16_tflops_sustained", 1400.0)
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = H100_BF16_TFLOPS
+    peak_src = "H100 SXM data sheet, dense BF16 (700 W)"
     g_ms, g_flop, g_n = gemm_t.result()
     a_ms, a_flop, a_n = attn_t.result()
     d_ms, d_flop, d_n = attn_d.result()
     step_ms_total = ms_step * args.steps
-    traffic = load_traffic()
 
     def fam(name, kernel, ms, flop, n, flop_model):
         ach = flop / ms / 1e9 if ms else None
-        t = traffic.get(name, {})
         return {"name": name, "kernel": kernel, "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s",
                 "frac": ach / peak_tf if ach else None, "launches_timed": n, "share_of_step": ms / step_ms_total if ms else None,
-                "flop_model": flop_model, "traffic": t.get("dram_bytes_per_launch"),
-                "algorithmic_bytes": t.get("algorithmic_bytes_per_launch"), "traffic_source": t.get("source")}
+                "flop_model": flop_model}
 
     kernels = [fam("gemm", "fvb::gemm_bf16_kernel (every linear of the step)", g_ms, g_flop, g_n, "2*M*N*K"),
-               fam("attention_sparse", "fvb::attn_ws_r1_kernel (VSA sparse branch, per-q-block lists; fvb::attn_ws_kernel under FVB_ATTN_IMPL=r2)", a_ms, a_flop, a_n,
+               fam("attention_sparse", "fvb::attn_fwd_kernel (VSA sparse branch, per-q-block lists)", a_ms, a_flop, a_n,
                    "4*B*H*S_q*topk*64*d (reference bench_vsa.py:84-86)"),
                fam("attention_dense", "fvb::attn_fwd_kernel (cross attention; self attention of dense workloads)", d_ms, d_flop, d_n,
                    "4*B*H*S_q*S_kv*d")]
@@ -506,7 +507,7 @@ def run_gpu_arm(args, rank, world, device):
     if kernels and kernels[0]["name"] == "gemm":
         kernels[0]["shapes"] = gemm_t.by_tag()[:8]
     r_ms, r_bytes, r_n = rows_t.result()
-    hbm_peak = (peaks or {}).get("hbm_gbs")
+    hbm_peak = H100_HBM_GBS
     r_gbs = r_bytes / r_ms / 1e6 if r_ms else None
     kernels.append({"name": "rows_and_index",
                     "kernel": "LayerNorm / RMSNorm+RoPE / block means / coarse softmax / top-k + list / gate combine kernels",
@@ -520,7 +521,6 @@ def run_gpu_arm(args, rank, world, device):
     # contract object = the dominant family (largest share of the step); every family sits in roofline.kernels
     roof = {"bound": "tensor", "kernel": dom["kernel"] if dom else None, "achieved": dom["achieved"] if dom else None,
             "peak": peak_tf, "peak_source": peak_src, "unit": "TFLOP/s", "frac": dom["frac"] if dom else None,
-            "traffic": dom.get("traffic") if dom else None, "algorithmic_bytes": dom.get("algorithmic_bytes") if dom else None,
             "launches_timed": dom["launches_timed"] if dom else 0, "share_of_step": dom["share_of_step"] if dom else None,
             "kernels": kernels}
     roof_attn = next((k for k in kernels if k["name"] == "attention_sparse"), None) or next(
@@ -587,6 +587,8 @@ def main():
     ap.add_argument("--layers", type=int, default=0, help="development only: truncate the model (result is flagged)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-sizes", default="", help="CPU arm: comma-separated token counts of the block samples")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's output as float32 .npy files under DIR")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -32,21 +32,6 @@ def lib() -> ctypes.CDLL:
     return _lib
 
 
-_probe = None
-
-
-def probe_lib() -> ctypes.CDLL:
-    """libfvb200_probe.so: hardware probes (include/fvb200_probe.h), used by tools/ only."""
-    global _probe
-    if _probe is None:
-        path = _PKG / "libfvb200_probe.so"
-        if not path.exists():
-            raise FvbError(f"{path} is missing: run `python -m fastvideo_b200.build`")
-        _probe = ctypes.CDLL(str(path))
-        _probe.fvb_probe_last_error.restype = c_char_p
-    return _probe
-
-
 LAUNCHES = 0  # kernels launched through the C ABI by this process (every fvb_* compute call launches one)
 
 

@@ -1,6 +1,6 @@
-"""Builds fastvideo_b200/libfvb200.so (all CUDA sources, sm_100a only) with nvcc.
+"""Builds fastvideo_b200/libfvb200.so (all CUDA sources, sm_90a only) with nvcc.
 
-Cross-compiles without a GPU. The .so is kept in-tree (git-ignored) so it travels to the GPU box.
+Cross-compiles without a GPU. The .so and the object cache are kept in-tree and git-ignored.
 """
 from __future__ import annotations
 
@@ -15,10 +15,9 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 OBJ = PKG.parent / "build" / "obj"
 LIB = PKG / "libfvb200.so"
-PROBE_LIB = PKG / "libfvb200_probe.so"  # hardware probes: separate library, not the product ABI
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wno-format-truncation",
     "-Xptxas", "-warn-spills",
 ]
@@ -42,7 +41,7 @@ def _digest(src: Path) -> str:
 
 def _compile(src: Path) -> Path:
     OBJ.mkdir(parents=True, exist_ok=True)
-    tag = src.stem if src.parent == CSRC else f"{src.parent.name}_{src.stem}"
+    tag = src.stem
     obj = OBJ / (tag + ".o")
     stamp = OBJ / (tag + ".sha")
     dg = _digest(src)
@@ -68,17 +67,8 @@ def build(verbose: bool = True) -> Path:
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
-    psrcs = sorted((CSRC / "probe").glob("*.cu"))
-    if psrcs:
-        pobjs = [_compile(s) for s in psrcs]
-        if not PROBE_LIB.exists() or PROBE_LIB.stat().st_mtime < max(o.stat().st_mtime for o in pobjs):
-            r = subprocess.run([_nvcc(), "-shared", "-o", str(PROBE_LIB), *map(str, pobjs), "-cudart", "static"],
-                               capture_output=True, text=True)
-            if r.returncode != 0:
-                raise RuntimeError(f"probe link failed:\n{r.stdout}\n{r.stderr}")
     if verbose:
-        print(f"[fastvideo_b200.build] {LIB} ({LIB.stat().st_size >> 10} KiB, {len(srcs)} sources)"
-              + (f" + {PROBE_LIB.name} ({len(psrcs)} probe sources)" if psrcs else ""))
+        print(f"[fastvideo_b200.build] {LIB} ({LIB.stat().st_size >> 10} KiB, {len(srcs)} sources)")
     return LIB
 
 

@@ -11,7 +11,7 @@ Parameter names are the reference's; the pinned dtype flow is bf16 parameters an
 which the reference's `e = scale_shift_table + temb` is bf16 and every modulation / gate op rounds to bf16 -- the
 kernels reproduce those rounding points (FVB_EPI_RESID_GATE_BF16R, fvb_layernorm_modulate round_ln = 3).
 
-B200-first differences that do not change results:
+Implementation differences that do not change results:
   * the fused QKV GEMM writes K and V straight into the cache rows (per-head column-block offsets of
     fvb_linear_bf16_sp), QK-RMSNorm + RoPE then runs in place on the cache rows: no roped_key / v copies;
   * eviction does not move memory. The reference shifts the non-sink part of the cache left by the evicted token

@@ -79,8 +79,8 @@ inline int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;  // H100 SXM
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }

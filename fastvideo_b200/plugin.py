@@ -214,7 +214,7 @@ def _define():
 
         @classmethod
         def get_min_capability(cls) -> int:
-            return 100
+            return 90
 
         @staticmethod
         def get_config_filenames() -> list[str]:
@@ -279,10 +279,15 @@ def load_wan_block(block: torch.nn.Module, cfg=None):
     return wan_dit.WanBlock(sd, "", cfg)
 
 
+def device_supported() -> bool:
+    """The library holds sm_90a code only, which runs on compute capability 9.0 (H100 / H800 / H200) and nowhere else."""
+    return torch.cuda.is_available() and tuple(torch.cuda.get_device_capability()) == (9, 0)
+
+
 def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, custom_ops: bool = True,
             force: bool | None = None):
     """Registers everything (idempotent). `force=True` routes the dense backend even when the current device is not
-    sm_100 (used by the CPU registration test); by default it follows FVB200_FORCE=1 or a (10, x) CUDA device."""
+    sm_90 (used by the CPU registration test); by default it follows FVB200_FORCE=1 or device_supported()."""
     global _state
     if _state is not None:
         return _state.ns
@@ -319,12 +324,12 @@ def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, c
                   AttentionBackendEnum[DENSE_BACKEND_NAME])
 
         def get_attn_backend_cls(cls, selected_backend, head_size, dtype):
-            on_b200 = force or (torch.cuda.is_available() and torch.cuda.get_device_capability()[0] == 10)
-            if (on_b200 and selected_backend in routed and head_size == 128 and dtype == torch.bfloat16
+            on_device = force or device_supported()
+            if (on_device and selected_backend in routed and head_size == 128 and dtype == torch.bfloat16
                     and os.environ.get("FVB200_ATTENTION", "1") != "0"):
                 return f"{__name__}.Fvb200AttentionBackend"
             if selected_backend is AttentionBackendEnum[DENSE_BACKEND_NAME]:
-                raise ValueError(f"{DENSE_BACKEND_NAME} supports bf16 with head_size 128 on sm_100 only")
+                raise ValueError(f"{DENSE_BACKEND_NAME} supports bf16 with head_size 128 on sm_90 only")
             return orig_fn(cls, selected_backend, head_size, dtype)
 
         patch(plat_cls, "get_attn_backend_cls", classmethod(get_attn_backend_cls))

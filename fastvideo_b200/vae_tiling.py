@@ -5,8 +5,8 @@ callback for the per-tile decoder ([B, C, T, h, w] -> [B, 3, 4(T-1)+1, 8h, 8w]).
 
 Where the reference uses it: `ParallelTiledVAE.decode` is what a VAE's decode falls through to when its feature cache is
 off; for Wan the cache is ON by default (fastvideo/configs/models/vaes/wanvae.py:73), so the default Wan decode is the
-un-tiled per-latent-frame loop that fastvideo_b200/wan_vae.py implements, and 180 GB of HBM never forces tiling at the
-shapes in BASELINE.json. This module is the multi-GPU / memory-bounded variant of row a21 (tiles dealt to ranks, one
+un-tiled per-latent-frame loop that fastvideo_b200/wan_vae.py implements, and at the shapes in BASELINE.json the
+un-tiled decode fits in the 80 GB of an H100. This module is the multi-GPU / memory-bounded variant of row a21 (tiles dealt to ranks, one
 all_gather, blended seams). Its caller is fastvideo_b200.wan_vae.WanVAEDecoder.decode_tiled, which supplies the cache-less
 per-tile decoder (AutoencoderKLWan._decode: 4T frames per tile) and Wan's wrappers around these methods (wanvae.py:1228-1247:
 `blend_num_frames *= 2` on the temporal paths, first three frames of every tiled result dropped).

@@ -35,7 +35,7 @@ class WanVAEConfig:
 
 
 # fused consumer-norm epilogue (fvb_conv3d_cl_norm); FVB_VAE_FUSE_NORM=0/1 overrides (A/B measurements)
-FUSE_NORM = os.environ.get("FVB_VAE_FUSE_NORM", "1") == "1"  # measured: 1080p x 17f decode 528 -> 509 ms (profiles/r2_gpu_session7.log)
+FUSE_NORM = os.environ.get("FVB_VAE_FUSE_NORM", "1") == "1"  # saves a read and a write of the activation per norm
 
 
 class _Conv:

@@ -1,4 +1,4 @@
-/* fvb200.h -- C ABI of libfvb200.so, the B200 (sm_100a) implementation of FastVideo's Wan DiT
+/* fvb200.h -- C ABI of libfvb200.so, the H100 (sm_90a) implementation of FastVideo's Wan DiT
  * denoising hot path and Wan VAE decode.
  *
  * Every entry point takes plain device pointers, sizes, element strides and a cudaStream_t (passed as
@@ -35,7 +35,7 @@ int fvb_abi_version(void);
 const char* fvb_last_error(void);
 
 /* --------------------------------------------------------------------------------------------
- * Linear layers (tcgen05 GEMM, TMA-fed, fused epilogues)
+ * Linear layers (wgmma GEMM, TMA-fed, fused epilogues)
  * Replaces: ReplicatedLinear.forward -> UnquantizedLinearMethod.apply -> F.linear
  *   (fastvideo/layers/linear.py:146-156, 293-300) plus the op that follows it in
  *   WanTransformerBlock.forward (fastvideo/models/dits/wanvideo.py:394-431):
@@ -164,13 +164,8 @@ int fvb_attention_fwd(const void* q, const void* k, const void* v, void* o, floa
                       const int32_t* q_len, int nqb, const int32_t* kv_off, const int32_t* kv_len, int nkb,
                       void* stream);
 
-/* Which implementation fvb_attention_blocklist_fwd dispatches to in this process: 1 = one CTA per q-block pair
- * (attn_ws_r1_sm100.cu, the default), 2 = persistent with K/V sharing (attn_ws_sm100.cu); FVB_ATTN_IMPL=r1|r2 overrides.
- * Introspection only (tests pin the default with it: a dispatch edit once silently re-routed every call to the slower kernel). */
-int fvb_attention_blocklist_impl(void);
-
-/* Block-list attention for 64-row q blocks with per-block key lists, on the weight-stationary M=64 tcgen05 path
- * (no list sharing between neighbouring q blocks needed). Consumes the reference's index format directly:
+/* Block-list attention for 64-row q blocks with per-block key lists (the two q blocks of a CTA merge their lists on the
+ * fly, so a key block both select is loaded once). Consumes the reference's index format directly:
  * q2k_idx int32 [.., nqb, cap] ascending kv block ids (first q2k_num[..] valid), q2k_num int32 [.., nqb]
  * (map_to_index, fastvideo-kernel/python/fastvideo_kernel/triton_kernels/index.py:106-144); idx_stride_b / idx_stride_h
  * in q blocks (0 = broadcast over batch / heads). Same q/k/v/o addressing, offsets, lengths, masking, LSE and
@@ -184,9 +179,8 @@ int fvb_attention_blocklist_fwd(const void* q, const void* k, const void* v, voi
                                 int64_t idx_stride_h, int cap, const int32_t* q_off, const int32_t* q_len, int nqb,
                                 const int32_t* kv_off, const int32_t* kv_len, int nkb, void* workspace,
                                 int64_t workspace_bytes, void* stream);
-/* Bytes of caller-allocated device workspace (256-byte aligned) fvb_attention_blocklist_fwd needs: the per-pair
- * [common | only-mine] reordering of the lists (the two q blocks of a CTA load the key blocks they share once), and the
- * per-CTA exchange scratch of the epilogue. index_rows = how many (batch, head) combinations carry their own lists. */
+/* Bytes of caller-allocated device workspace (256-byte aligned) fvb_attention_blocklist_fwd accepts. Kept for ABI
+ * compatibility only: the sm_90a kernel merges the two lists of a CTA while it walks them and uses no workspace. */
 int64_t fvb_attention_blocklist_workspace_bytes(int index_rows, int nqb, int cap);
 
 /* Backward of fvb_attention_blocklist_fwd in the padded layout (block i = rows [64 i, 64 i + 64)): dq, dk, dv from q, k, v, o,
@@ -194,7 +188,7 @@ int64_t fvb_attention_blocklist_workspace_bytes(int index_rows, int nqb, int cap
  * ascending, the q blocks that selected each kv block (the inverse lists, triton_kernels/index.py:147-250 invert_indices);
  * idx_stride_* / kidx_stride_* in rows of the respective index tensors (0 = broadcast). delta_ws: fp32 [B * H * Sq] workspace.
  * Replaces block_sparse_attn_backward_triton (fastvideo-kernel/python/fastvideo_kernel/block_sparse_attn.py:138-243;
- * triton_kernels/block_sparse_attn_triton.py:165-694). First implementation: warp-level mma.sync tiles (csrc/attn_bwd_sm100.cu). */
+ * triton_kernels/block_sparse_attn_triton.py:165-694). Warp-level mma.sync tiles (csrc/attn_bwd_sm90.cu). */
 int fvb_attention_blocklist_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
                                 void* dq, void* dk, void* dv, float* delta_ws, const int64_t* q_strides,
                                 const int64_t* k_strides, const int64_t* v_strides, const int64_t* o_strides,
@@ -294,7 +288,7 @@ int fvb_gather_rows(const void* in, int64_t in_batch_stride, int64_t in_ld, cons
 int fvb_gemm_f32out(const void* a, int64_t lda, const void* b, int64_t ldb, float* out, int64_t ldo, int M, int N, int K,
                     float scale, void* stream);
 
-/* Causal Conv3d / Conv2d as a TMA-staged implicit GEMM (tcgen05). Replaces WanCausalConv3d.forward
+/* Causal Conv3d / Conv2d as a TMA-staged implicit GEMM (wgmma). Replaces WanCausalConv3d.forward
  * (fastvideo/models/vaes/wanvae.py:160-207) and the Conv2d of WanResample (wanvae.py:272-281).
  *   x: [T_in][H][W][Cin] input frames: the (<= 2) cached frames of the feature cache followed by the new frames;
  *   t_off = number of cached frames present; output frame j (0 <= j < T_out) is computed from input frames
@@ -303,9 +297,7 @@ int fvb_gemm_f32out(const void* a, int64_t lda, const void* b, int64_t ldb, floa
  *   y = bf16(acc + bias); out = bf16(y + resid) if resid. out: [T_out][H][W][out_ld].
  *   interleave_c = Cout/2: output channel c of frame j goes to frame 2j + c / interleave_c, channel c % interleave_c
  *   (the reshape + stack after time_conv in upsample3d, wanvae.py:343-345; out must hold 2*T_out frames).
- *   Kernel selection is internal: 3x3 spatial kernels with Cout <= 128 take the halo-box variant (one activation box per
- *   (time tap, row tap, channel block) feeds the three column taps), everything else one box per tap; the two differ only
- *   in the order of the fp32 sums (FVB_CONV_WIDE=0 forces the per-tap kernel). */
+ *   One TMA box of activations per tap and channel block. */
 int fvb_conv3d_cl(const void* x, int T_in, int H, int W, int Cin, const void* w_packed, int Cin_pad, int Cout, int kt,
                   int kh, int kw, const void* bias, const void* resid, int64_t resid_ld, void* out, int64_t out_ld,
                   int T_out, int t_off, int interleave_c, void* stream);

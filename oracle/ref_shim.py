@@ -1,12 +1,12 @@
 """TEST INFRASTRUCTURE ONLY -- makes the reference's own Python importable on a CPU-only box.
 
-Only oracle/gen_golden.py (run in the build container, where /root/reference exists) uses this, to
-(a) validate the restatements in oracle/*.py against the reference itself and (b) write the small
-golden fixtures under tests/golden/. Nothing on the product path, in the -m gpu tests, in smoke() or
-in bench.py imports it: /root/reference does not exist on the GPU box.
+The reference tree is $FVB_REFERENCE_ROOT, else oracle/_ref/reference_py (staged by oracle/stage_ref_kernels.py,
+git-ignored). oracle/gen_golden.py uses this to (a) validate the restatements in oracle/*.py against the reference itself
+and (b) write the small golden fixtures under tests/golden/; tests/test_plugin_cpu.py uses it to register the plug-in into
+the reference. Nothing on the product path, in smoke() or in bench.py's GPU arm imports it.
 
 Recipe (SURVEY.md section 8c / Appendix A): register a bare `fastvideo` package whose __path__ points at
-/root/reference/fastvideo (skipping fastvideo/__init__.py, which pulls in imageio/diffusers via
+<reference root>/fastvideo (skipping fastvideo/__init__.py, which pulls in imageio/diffusers via
 VideoGenerator), stub the three missing third-party roots, point the CPU platform at the SDPA backend
 (fastvideo/platforms/interface.py:122-125 returns "" on CPU) and make get_local_torch_device() return
 cpu (fastvideo/distributed/parallel_state.py:881-890 maps non-CUDA to mps).
@@ -21,7 +21,9 @@ import socket
 import sys
 import types
 
-REF_ROOT = os.environ.get("FVB_REFERENCE_ROOT", "/root/reference")
+_HERE = os.path.dirname(os.path.abspath(__file__))
+# the reference's Python: $FVB_REFERENCE_ROOT, else the copy oracle/stage_ref_kernels.py stages into oracle/_ref/reference_py
+REF_ROOT = os.environ.get("FVB_REFERENCE_ROOT") or os.path.join(_HERE, "_ref", "reference_py")
 _STUB_ROOTS = {"imageio", "diffusers", "remote_pdb"}
 _installed = False
 
@@ -148,7 +150,7 @@ def install() -> None:
     from fastvideo.platforms.cpu import CpuPlatform
     CpuPlatform.get_attn_backend_cls = classmethod(
         lambda cls, sel, head_size, dtype: "fastvideo.attention.backends.sdpa.SDPABackend")
-    # The shim is the reference's CPU path by definition. On a box that HAS a GPU (bench.py's CPU arm on the B200 host)
+    # The shim is the reference's CPU path by definition. On a box that HAS a GPU (bench.py's CPU arm on the GPU host)
     # the reference would resolve CudaPlatform through NVML (fastvideo/platforms/__init__.py:16-49); pin the CPU platform.
     import fastvideo.platforms as _plat
     if not isinstance(getattr(_plat, "_current_platform", None), CpuPlatform):

@@ -12,7 +12,7 @@ Run in the build container:  python -m oracle.stage_ref_kernels
 import os
 import shutil
 
-REF = os.environ.get("FVB_REFERENCE_ROOT", "/root/reference")
+REF = os.environ.get("FVB_REFERENCE_ROOT", "")
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(REF, "fastvideo-kernel", "python", "fastvideo_kernel")
 DST = os.path.join(HERE, "_ref", "fastvideo_kernel")

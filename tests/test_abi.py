@@ -46,13 +46,13 @@ def test_product_never_imports_oracle():
                 assert "/root/reference" not in src, f
 
 
-def test_default_block_list_attention_kernel_is_r1():
-    """The VSA sparse branch must dispatch to the kernel the committed head-to-heads selected (profiles/r2_k1_headtohead_*)."""
-    import os
-    import subprocess
-    import sys
-    code = "from fastvideo_b200._lib import lib; print(lib().fvb_attention_blocklist_impl())"
-    env = {k: v for k, v in os.environ.items() if k != "FVB_ATTN_IMPL"}
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=ROOT, env=env)
-    assert out.returncode == 0, out.stderr[-500:]
-    assert out.stdout.strip() == "1"
+def test_plugin_routes_only_on_compute_capability_9_0(monkeypatch):
+    """The library holds sm_90a code: the plug-in points route to it on a (9, 0) device and on nothing else."""
+    import torch
+    from fastvideo_b200 import plugin
+    monkeypatch.setattr(torch.cuda, "is_available", lambda: True)
+    for cap, want in (((9, 0), True), ((10, 0), False), ((8, 0), False), ((9, 1), False)):
+        monkeypatch.setattr(torch.cuda, "get_device_capability", lambda *a, cap=cap: cap)
+        assert plugin.device_supported() is want, cap
+    monkeypatch.setattr(torch.cuda, "is_available", lambda: False)
+    assert plugin.device_supported() is False

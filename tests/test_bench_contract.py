@@ -8,10 +8,10 @@ import sys
 from conftest import ROOT
 
 
-def test_reference_arm_prints_one_json_line():
+def test_reference_arm_prints_one_json_line(tmp_path):
     env = dict(os.environ, OMP_NUM_THREADS="8")
     p = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "0",
-                        "--cpu-sizes", "256,512"],
+                        "--cpu-sizes", "256,512", "--dump-outputs", str(tmp_path / "dump")],
                        capture_output=True, text=True, timeout=600, cwd=ROOT, env=env)
     assert p.returncode == 0, p.stderr[-2000:]
     lines = [l for l in p.stdout.splitlines() if l.strip()]
@@ -27,6 +27,9 @@ def test_reference_arm_prints_one_json_line():
     ex = d["config"]["extrapolation"]
     assert ex["S"] == d["config"]["tokens"] == 75600 and ex["a"] > 0 and "S in" in d["cpu_baseline"]["sample"]
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
+    import numpy as np
+    dumped = np.load(tmp_path / "dump" / "block_output.npy")  # the last timed block: [1, 512 tokens, D], float32
+    assert dumped.dtype == np.float32 and dumped.shape[-2:] == (512, 5120) and np.isfinite(dumped).all()
 
 
 def test_gpu_arm_refuses_to_run_without_cuda():

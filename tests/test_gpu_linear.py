@@ -1,4 +1,4 @@
-"""GPU: tcgen05 GEMM + fused epilogues against an fp32 torch reference of the same op (rounding mirrored)."""
+"""GPU: wgmma GEMM + fused epilogues against an fp32 torch reference of the same op (rounding mirrored)."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -4,14 +4,14 @@ Runs the reference's own selector / registry / module constructors (imported thr
 they resolve to the libfvb200 classes, that the ABC contracts hold (the classes instantiate), that a reference
 `ReplicatedLinear` accepts the LinearMethodBase, and that a reference WanTransformerBlock's state_dict() loads into
 wan_dit.WanBlock. No compute is run (no GPU here): with CPU tensors the ops raise FvbError, which is asserted too.
-Skipped where /root/reference is absent (the GPU box).
+Skipped where the reference tree is absent ($FVB_REFERENCE_ROOT, else oracle/_ref/reference_py).
 """
 import pytest
 import torch
 
 from oracle import ref_shim
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present (GPU box)")
+pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not present (set FVB_REFERENCE_ROOT or stage oracle/_ref/reference_py)")
 
 
 @pytest.fixture(scope="module")

@@ -41,4 +41,4 @@ res["fused_compact_union"] = timed(lambda: ops.attention(qv, kv_, vv, out=o2, sc
 q3, k3, v3 = (torch.randn(1, S, H, 128, device="cuda", dtype=torch.bfloat16) for _ in range(3))
 res["bshd_compact_ws"] = timed(lambda: ops.attention_blocklist(q3, k3, v3, idx, num, out=o2, q_off=off, kv_off=off, q_len=vbs, kv_len=vbs, nkb=nb))
 print(json.dumps(res))
-json.dump(res, open("gpurun_out/attn_layouts.json", "w"), indent=1)
+json.dump(res, open("tool_out/attn_layouts.json", "w"), indent=1)

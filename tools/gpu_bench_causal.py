@@ -1,4 +1,4 @@
-"""Causal (self-forcing) Wan rollout step on B200 -- BASELINE.json config #4 geometry: Wan 14B widths, 480x832 latents
+"""Causal (self-forcing) Wan rollout step on H100 -- BASELINE.json config #4 geometry: Wan 14B widths, 480x832 latents
 (60x104 -> 30x52 = 1560 tokens per latent frame), 3-frame blocks (4680 query tokens) against a 21-frame KV window
 (32 760 keys), random-init weights, synthetic latents. One "step" = one CausalWanDiT.forward_inference call (all 40
 layers) for one frame block at one denoising timestep. Reports ms/step at (a) the full window with in-place overwrite
@@ -64,7 +64,7 @@ def main():
                frac_of_sustained_bf16_peak=flop / med(ms_same) / 1e9 / 1447.0,
                peak_mem_gib=torch.cuda.max_memory_allocated() / 2 ** 30, finite=True)
     print(json.dumps(res))
-    json.dump(res, open("gpurun_out/causal_bench.json", "w"), indent=1)
+    json.dump(res, open("tool_out/causal_bench.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Wan VAE decode throughput on B200 (BASELINE.json config #5 geometry: 1080p latent 135x240, 8x spatial / 4x temporal),
+"""Wan VAE decode throughput on H100 (BASELINE.json config #5 geometry: 1080p latent 135x240, 8x spatial / 4x temporal),
 random-init decoder at the real widths (base_dim 96). Reports output voxels/s, TFLOP/s against the 8.44 MFLOP/voxel
 model and GB/s against the 5.59 KB/voxel unfused-conv traffic model (SURVEY.md section 8d)."""
 import json, sys, time
@@ -59,7 +59,7 @@ def main():
     res = dict(latent=[T, h, w], out=list(y.shape), iters=iters, ms_all=[round(t, 2) for t in times], ms=ms, voxels_per_s=vox / ms * 1e3, tflops_model=vox * 8.44e6 / ms / 1e9,
                gbs_unfused_model=vox * 5.59e3 / ms / 1e6, finite=bool(torch.isfinite(y).all()), peak_mem_gib=torch.cuda.max_memory_allocated() / 2**30)
     print(json.dumps(res))
-    json.dump(res, open(f"gpurun_out/vae_bench_T{T}.json", "w"), indent=1)
+    json.dump(res, open(f"tool_out/vae_bench_T{T}.json", "w"), indent=1)
 
 if __name__ == "__main__":
     main()

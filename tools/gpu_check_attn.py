@@ -1,4 +1,4 @@
-"""GPU check of the attention kernel and the row kernels against fp32 torch (run under gpurun)."""
+"""GPU check of the attention kernel and the row kernels against fp32 torch."""
 import sys, math, json, time
 import numpy as np
 import torch

@@ -1,4 +1,4 @@
-"""GPU check of the tcgen05 GEMM against torch (run under gpurun)."""
+"""GPU check of the wgmma GEMM against torch."""
 import sys, time, json
 import torch
 sys.path.insert(0, ".")
@@ -61,7 +61,7 @@ def main():
         ms_t = e0.elapsed_time(e1) / 10
         print(f"time M={M} N={N} K={K} epi={epi}: {ms:.3f} ms = {tf:.0f} TFLOP/s | cuBLAS F.linear {ms_t:.3f} ms = {2*M*N*K/ms_t/1e9:.0f} TFLOP/s", flush=True)
         res.append(dict(M=M, N=N, K=K, epi=epi, ms=ms, tflops=tf, cublas_ms=ms_t))
-    json.dump(res, open("gpurun_out/gemm_check.json", "w"), indent=1)
+    json.dump(res, open("tool_out/gemm_check.json", "w"), indent=1)
 
 if __name__ == "__main__":
     main()

@@ -22,5 +22,5 @@ for name, N, K, epi in shapes:
     res["cases"].append(dict(name=name, N=N, K=K, ms=ms, tflops=2.0 * S * N * K / ms / 1e9))
     del x, w, resid
 print(json.dumps(res))
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(res, open(f"gpurun_out/gemm_shapes_S{S}_stripe{res['stripe']}.json", "w"), indent=1)
+os.makedirs("tool_out", exist_ok=True)
+json.dump(res, open(f"tool_out/gemm_shapes_S{S}_stripe{res['stripe']}.json", "w"), indent=1)

@@ -22,5 +22,5 @@ res["topk_index_ms"] = timed(lambda: ops.topk_index(s, 144))
 res["bytes_scores_plus_lists"] = s.numel() * 2 + s.numel() * 4
 res["topk_index_tb_s"] = res["bytes_scores_plus_lists"] / res["topk_index_ms"] / 1e9
 print(json.dumps(res))
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(res, open(f"gpurun_out/index_time_warp{res['topk_warp']}.json", "w"), indent=1)
+os.makedirs("tool_out", exist_ok=True)
+json.dump(res, open(f"tool_out/index_time_warp{res['topk_warp']}.json", "w"), indent=1)

@@ -27,4 +27,4 @@ res["rmsnorm_q_only"] = timed(lambda: ops.rmsnorm_rope_(x, nw, head_dim=128))
 gb = {"ln_bf16_mod": 2 * S * D * 2, "ln_bf16_round_mod": 2 * S * D * 2, "ln_f32_affine_hidden": S * D * (4 + 2 + 2), "rmsnorm_rope_qk": 4 * S * D * 2, "rmsnorm_q_only": 2 * S * D * 2}
 out = {k: dict(ms=v, tb_s=gb[k] / v / 1e9) for k, v in res.items()}
 print(json.dumps(out))
-os.makedirs("gpurun_out", exist_ok=True); json.dump(out, open("gpurun_out/rowops_time.json", "w"), indent=1)
+os.makedirs("tool_out", exist_ok=True); json.dump(out, open("tool_out/rowops_time.json", "w"), indent=1)
