@@ -51,11 +51,11 @@ inline EncodeTiledFn get_encode_tiled() {
   return fn;
 }
 
-// bf16 tensor map of rank `rank` (<= 5). dims/strides innermost first; strides[0] is implied
-// (2 bytes) and strides[i] (bytes) must be multiples of 16. 128B swizzle, zero OOB fill.
-inline int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                          const uint64_t* strides_bytes, const uint32_t* box,
-                          CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+// Tensor map of rank `rank` (<= 5) over elements of type `dtype`. dims/strides innermost first; strides[0] is implied
+// (one element) and strides[i] (bytes) must be multiples of 16. 128B swizzle by default, zero OOB fill.
+inline int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box,
+                     CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn enc = get_encode_tiled();
   if (!enc) return set_error(FVB_ERR_NO_DEVICE, "cuTensorMapEncodeTiled unavailable (no CUDA driver)%s");
   cuuint64_t gdim[5], gstr[4];
@@ -68,11 +68,25 @@ inline int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const ui
   }
   if ((reinterpret_cast<uintptr_t>(base) & 15) != 0)
     return set_error(FVB_ERR_INVALID_ARG, "tensor base not 16B aligned%s");
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim,
+  CUresult r = enc(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim,
                    gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(FVB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%s) code %lld", "", (long long)r);
   return FVB_OK;
+}
+
+// bf16 tensor map (strides[0] implied: 2 bytes)
+inline int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                          const uint64_t* strides_bytes, const uint32_t* box,
+                          CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box, swz);
+}
+
+// one-byte tensor map (fp8 e4m3 operands; strides[0] implied: 1 byte)
+inline int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                        const uint64_t* strides_bytes, const uint32_t* box,
+                        CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+  return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, swz);
 }
 
 inline int sm_count() {

@@ -1,7 +1,11 @@
-// gemm_sm90.cu -- persistent, warp-specialised bf16 GEMM for sm_90a:
-//   out = epilogue(x[M,K] @ w[N,K]^T + bias)
+// gemm_sm90.cu -- persistent, warp-specialised GEMM for sm_90a, bf16 or fp8 (e4m3) operands:
+//   out = epilogue(x[M,K] @ w[N,K]^T + bias)                                   (bf16)
+//   out = epilogue((x_q[M,K] @ w_q[N,K]^T) * x_scale[m] * w_scale[n] + bias)   (e4m3, per-row / per-channel scales)
 // TMA (128B swizzle) -> shared-memory ring -> wgmma (two warpgroups, 64 rows x BN each, fp32 accumulators in registers)
 // -> epilogue straight from the accumulator registers with fused bias / GELU(tanh) / gated residual.
+// A k-block is one 128-byte swizzle row of both operands: 64 bf16 or 128 e4m3 elements, so a stage holds the same bytes
+// for both types. The e4m3 tensor-core accumulator keeps fewer bits than fp32, so the fp8 path lets each k-block's MMAs
+// accumulate into a second register set and adds that into the fp32 accumulators once per k-block (every 128 elements).
 //
 // Stands behind fastvideo/layers/linear.py:146-156 (F.linear) and the elementwise op that follows
 // each linear in fastvideo/models/dits/wanvideo.py:394-431; rounding points mirror the reference's
@@ -14,6 +18,7 @@
 // the row-blocks stream past it. Output column blocks may be redirected by an offset table (out_col_offsets), which
 // is how the sequence-parallel paths write heads straight into send / peer receive buffers.
 #include <cstdlib>
+#include <type_traits>
 #include "fvb_host.cuh"
 #include "fvb_ptx.cuh"
 
@@ -21,6 +26,7 @@ namespace fvb {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;   // 64 bf16 = one 128B swizzle row
+constexpr int GEMM_BK_FP8 = 128;  // 128 e4m3 = one 128B swizzle row
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_GROUP_M = 8;
 
@@ -41,6 +47,15 @@ struct GemmParams {
   int batch;
   int stripe_n;  // > 0: weight-stripe raster with this many column tiles per stripe (see tile_coords)
 };
+
+// e4m3 operands: the per-row / per-channel scales. The bf16 kernels keep taking the plain GemmParams.
+struct GemmParamsFp8 : GemmParams {
+  const float* a_scale;  // [M]
+  const float* b_scale;  // [N_valid]
+  int N_valid;           // columns with a b_scale entry (N before rounding up to 8)
+};
+template <bool FP8>
+using GemmParamsT = std::conditional_t<FP8, GemmParamsFp8, GemmParams>;
 
 template <int BN>
 struct GemmCfg {
@@ -85,11 +100,11 @@ FVB_DEVICE float gelu_tanh_f(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool FP8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8> p) {
   using Cfg = GemmCfg<BN>;
+  constexpr int BK = FP8 ? GEMM_BK_FP8 : GEMM_BK;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
@@ -127,11 +142,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           uint8_t* sb = sa + Cfg::A_BYTES;
           mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
           {
-            const int k0 = kb * GEMM_BK;
+            const int k0 = kb * BK;
             const int seg = k0 / p.a_seg_len;
             tma_load_4d(sa, &tmA, &full[stage], k0 - seg * p.a_seg_len, m_blk * GEMM_BM, seg, bt);
           }
-          tma_load_3d(sb, &tmB, &full[stage], kb * GEMM_BK, n_blk * BN, bt);
+          tma_load_3d(sb, &tmB, &full[stage], kb * BK, n_blk * BN, bt);
           if (++stage == Cfg::STAGES) {
             stage = 0;
             phase ^= 1;
@@ -156,6 +171,33 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int prev = -1;
+    if constexpr (FP8) {
+      // per k-block partial sums in `part` (the first MMA overwrites it), promoted into the fp32 accumulators after the
+      // k-block's MMAs complete; the other consumer warpgroup keeps the tensor cores busy meanwhile
+      float part[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
+      for (int kb = 0; kb < p.num_k; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + half * (64 * 128);
+        const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+        const uint64_t da = make_desc_kmajor_sw128(sa);
+        const uint64_t db = make_desc_kmajor_sw128(sb);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK_FP8 / 32; ++k) wgmma_ss_e4m3<BN>(part, da + uint64_t(2 * k), db + uint64_t(2 * k), k);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(part);
+        if (lane == 0) mbar_arrive(&empty[stage]);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = __fadd_rn(acc[i], part[i]);
+        if (++stage == Cfg::STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    } else {
     for (int kb = 0; kb < p.num_k; ++kb) {
       mbar_wait(&full[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + half * (64 * 128);
@@ -178,6 +220,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    }
 
     // ------------------------------ epilogue ------------------------------
     const int row0 = m_blk * GEMM_BM + half * 64 + warp * 16 + (lane >> 2);
@@ -185,6 +228,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if constexpr (EPI != FVB_EPI_RESID_BF16)
       if (p.gate_rows > 0)
         for (int i = 0; i < 2; ++i) gate_rows_p[i] += int64_t((row0 + 8 * i) / p.gate_rows) * p.gate_stride;
+    float sx[2] = {1.f, 1.f};
+    if constexpr (FP8)
+      for (int i = 0; i < 2; ++i) sx[i] = row0 + 8 * i < p.M ? __ldg(p.a_scale + row0 + 8 * i) : 0.f;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       const int col = n_blk * BN + 8 * j + 2 * (lane & 3);
@@ -192,11 +238,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int64_t out_col = p.out_col_offsets ? __ldg(p.out_col_offsets + (col >> 7)) + (col & 127) : int64_t(col);
       float2 bf = make_float2(0.f, 0.f);
       if (p.bias != nullptr) bf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
+      float2 sw = make_float2(1.f, 1.f);
+      if constexpr (FP8) {
+        sw.x = col < p.N_valid ? __ldg(p.b_scale + col) : 0.f;
+        sw.y = col + 1 < p.N_valid ? __ldg(p.b_scale + col + 1) : 0.f;
+      }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int row = row0 + 8 * i;
         if (row >= p.M) continue;
         float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
+        if constexpr (FP8) {  // (acc * s_x[m]) * s_w[n], fp32 round-to-nearest, before the bias
+          f0 = __fmul_rn(__fmul_rn(f0, sx[i]), sw.x);
+          f1 = __fmul_rn(__fmul_rn(f1, sx[i]), sw.y);
+        }
         if (p.bias != nullptr) {
           f0 = __fadd_rn(f0, bf.x);
           f1 = __fadd_rn(f1, bf.y);
@@ -241,10 +296,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-template <int BN, int EPI>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+template <int BN, int EPI, bool FP8>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8>& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<BN, EPI>;
+  auto kern = gemm_kernel<BN, EPI, FP8>;
   static bool configured = false;
   if (!configured) {
     FVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -260,16 +315,30 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
 template <int BN>
 static int dispatch_epi(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, cudaStream_t st) {
   switch (epi) {
-    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS>(a, b, p, st);
-    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R>(a, b, p, st);
-    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16>(a, b, p, st);
-    case FVB_EPI_DIV: return launch_gemm<BN, FVB_EPI_DIV>(a, b, p, st);
-    case FVB_EPI_SCALE_F32: return launch_gemm<BN, FVB_EPI_SCALE_F32>(a, b, p, st);
+    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, false>(a, b, p, st);
+    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, false>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, false>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, false>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, false>(a, b, p, st);
+    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, false>(a, b, p, st);
+    case FVB_EPI_DIV: return launch_gemm<BN, FVB_EPI_DIV, false>(a, b, p, st);
+    case FVB_EPI_SCALE_F32: return launch_gemm<BN, FVB_EPI_SCALE_F32, false>(a, b, p, st);
   }
   return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue%s");
+}
+
+// fp8 operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
+template <int BN>
+static int dispatch_epi_fp8(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsFp8& p, cudaStream_t st) {
+  switch (epi) {
+    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, true>(a, b, p, st);
+    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, true>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, true>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, true>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, true>(a, b, p, st);
+    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, true>(a, b, p, st);
+  }
+  return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue for fvb_linear_fp8%s");
 }
 
 }  // namespace fvb
@@ -280,9 +349,16 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
                      const void* bias, void* out, int64_t ldo, int64_t o_batch, const int64_t* out_col_offsets,
                      const void* resid, int64_t ldr,
                      const float* gate, int gate_rows, int64_t gate_stride, float div, int M, int N, int K, int batch,
-                     int epilogue, void* stream) {
+                     int epilogue, void* stream, const float* x_scale = nullptr, const float* w_scale = nullptr) {
+  // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales
+  const bool fp8 = x_scale != nullptr;
   FVB_CHECK_ARG(x && w && out, "null pointer");
   FVB_CHECK_ARG(M > 0 && N > 0 && K > 0 && batch > 0, "empty problem");
+  if (fp8) {
+    FVB_CHECK_ARG(w_scale != nullptr, "w_scale required");
+    FVB_CHECK_ARG(batch == 1 && a_seg_len <= 0 && out_col_offsets == nullptr, "fp8 operands: plain row-major, unbatched");
+    FVB_CHECK_ARG(ldx % 16 == 0 && ldw % 16 == 0, "fp8 ldx/ldw must be multiples of 16 (16-byte rows)");
+  }
   FVB_CHECK_ARG(ldx % 8 == 0 && ldw % 8 == 0 && ldo % 8 == 0, "ldx/ldw/ldo must be multiples of 8");
   // N not a multiple of 8: the tail columns up to the next multiple of 8 are written as zeros (they must fit in ldo)
   const int N_store = (N + 7) & ~7;
@@ -301,31 +377,35 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     }
   }
   if (epilogue == FVB_EPI_DIV) FVB_CHECK_ARG(div != 0.f, "divisor must be non-zero");
-  const int BN = (N >= 256 && N % 256 == 0) ? 256 : (N >= 128 && N % 128 == 0 ? 128 : (N >= 192 ? 256 : 64));
+  // fp8: the promotion registers double the accumulator footprint, so 128 columns is the widest tile that fits
+  const int BN = fp8 ? (N >= 128 ? 128 : 64)
+                     : (N >= 256 && N % 256 == 0) ? 256 : (N >= 128 && N % 128 == 0 ? 128 : (N >= 192 ? 256 : 64));
+  const int BK = fp8 ? GEMM_BK_FP8 : GEMM_BK;
+  const int esz = fp8 ? 1 : 2;  // operand element bytes
 
   CUtensorMap tmA, tmB;
   if (a_seg_len <= 0 || a_seg_len >= K) {
     a_seg_len = K;
-    a_seg_stride = 16;  // unused (single segment); any 16B multiple
+    a_seg_stride = 16;  // unused (single segment); any multiple of 16 elements
   }
   FVB_CHECK_ARG(a_seg_len % GEMM_BK == 0 || a_seg_len == K, "A segment length must be a multiple of 64");
   FVB_CHECK_ARG(K % a_seg_len == 0 && a_seg_stride % 8 == 0, "bad A segmentation");
   {
     uint64_t dims[4] = {(uint64_t)a_seg_len, (uint64_t)M, (uint64_t)(K / a_seg_len), (uint64_t)batch};
-    uint64_t str[4] = {2, (uint64_t)ldx * 2, (uint64_t)a_seg_stride * 2,
-                       (uint64_t)(batch > 1 ? x_batch : 8) * 2};
-    uint32_t box[4] = {GEMM_BK, GEMM_BM, 1, 1};
-    int r = make_tmap_bf16(&tmA, x, 4, dims, str, box);
+    uint64_t str[4] = {(uint64_t)esz, (uint64_t)ldx * esz, (uint64_t)a_seg_stride * esz,
+                       batch > 1 ? (uint64_t)x_batch * esz : 16};  // unused dimension (size 1): any 16-byte multiple
+    uint32_t box[4] = {(uint32_t)BK, GEMM_BM, 1, 1};
+    int r = fp8 ? make_tmap_u8(&tmA, x, 4, dims, str, box) : make_tmap_bf16(&tmA, x, 4, dims, str, box);
     if (r) return r;
   }
   {
     uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)batch};
-    uint64_t str[3] = {2, (uint64_t)ldw * 2, (uint64_t)(batch > 1 ? w_batch : ldw * (int64_t)N) * 2};
-    uint32_t box[3] = {GEMM_BK, (uint32_t)BN, 1};
-    int r = make_tmap_bf16(&tmB, w, 3, dims, str, box);
+    uint64_t str[3] = {(uint64_t)esz, (uint64_t)ldw * esz, (uint64_t)(batch > 1 ? w_batch : ldw * (int64_t)N) * esz};
+    uint32_t box[3] = {(uint32_t)BK, (uint32_t)BN, 1};
+    int r = fp8 ? make_tmap_u8(&tmB, w, 3, dims, str, box) : make_tmap_bf16(&tmB, w, 3, dims, str, box);
     if (r) return r;
   }
-  GemmParams p;
+  GemmParamsFp8 p;  // the bf16 kernels receive its GemmParams part
   p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   p.out = out;
   p.resid = reinterpret_cast<const __nv_bfloat16*>(resid);
@@ -338,13 +418,16 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
   p.out_col_offsets = out_col_offsets;
   p.a_seg_len = a_seg_len;
   p.div = div;
+  p.a_scale = x_scale;
+  p.b_scale = w_scale;
+  p.N_valid = N;
   p.M = M;
   p.N = N_store;
   p.K = K;
   p.batch = batch;
   p.num_m = (M + GEMM_BM - 1) / GEMM_BM;
   p.num_n = (N + BN - 1) / BN;
-  p.num_k = (K + GEMM_BK - 1) / GEMM_BK;
+  p.num_k = (K + BK - 1) / BK;
   static const int stripe_env = [] { const char* e = getenv("FVB_GEMM_STRIPE_N"); return e ? atoi(e) : -1; }();
   // default: stripes of 8 column tiles once the problem is tall enough for a stripe sweep to fill several waves
   p.stripe_n = stripe_env >= 0 ? stripe_env : 8;
@@ -354,6 +437,7 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     p.stripe_n = 0;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (fp8) return BN == 128 ? dispatch_epi_fp8<128>(epilogue, tmA, tmB, p, st) : dispatch_epi_fp8<64>(epilogue, tmA, tmB, p, st);
   if (BN == 256) return dispatch_epi<256>(epilogue, tmA, tmB, p, st);
   if (BN == 128) return dispatch_epi<128>(epilogue, tmA, tmB, p, st);
   return dispatch_epi<64>(epilogue, tmA, tmB, p, st);
@@ -388,4 +472,13 @@ extern "C" int fvb_gemm_f32out(const void* a, int64_t lda, const void* b, int64_
                                int K, float scale, void* stream) {
   return gemm_impl(a, lda, 0, 0, 0, b, ldb, 0, nullptr, out, ldo, 0, nullptr, nullptr, 0, nullptr, 0, 0, scale, M, N, K, 1,
                    FVB_EPI_SCALE_F32, stream);
+}
+
+extern "C" int fvb_linear_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw,
+                              const float* w_scale, const void* bias, void* out, int64_t ldo, const void* resid, int64_t ldr,
+                              const float* gate, int gate_rows, int64_t gate_stride, int M, int N, int K, int epilogue,
+                              void* stream) {
+  if (x_scale == nullptr || w_scale == nullptr) return set_error(FVB_ERR_INVALID_ARG, "invalid argument: x_scale and w_scale are required%s");
+  return gemm_impl(xq, ldx, 0, 0, 0, wq, ldw, 0, bias, out, ldo, 0, nullptr, resid, ldr, gate, gate_rows, gate_stride, 1.0f,
+                   M, N, K, 1, epilogue, stream, x_scale, w_scale);
 }

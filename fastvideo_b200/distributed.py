@@ -153,6 +153,9 @@ class SPWanDiT:
     """WanDiT sharded over `world` ranks. Every rank holds all weights (replicated, as in the reference)."""
 
     def __init__(self, model, rank: int, world: int, group=None, comm: str | None = None):
+        if model.cfg.fp8_linears:
+            from ._lib import FvbError
+            raise FvbError("sequence parallelism runs bf16 linears only: build the model with fp8_linears=False")
         self.m = model
         self.rank, self.world, self.group = rank, world, group
         self._plans: dict = {}

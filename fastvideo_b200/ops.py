@@ -60,6 +60,96 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, e
     return out.reshape(*x.shape[:-1], N)
 
 
+FP8_E4M3_MAX = 448.0
+
+
+def quantize_fp8_rows(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """fvb_quantize_fp8_rows: bf16 [M, K] (rows may be strided; K % 8 == 0) -> (q float8_e4m3fn [M, K], scale fp32 [M])
+    with x[r] ~= q[r] * scale[r]. q's row stride is K rounded up to 16 (16-byte rows, what fvb_linear_fp8 loads)."""
+    _require_cuda_bf16(x, "x")
+    if x.dim() != 2 or x.stride(1) != 1:
+        raise FvbError("x must be a 2-D view with unit inner stride")
+    M, K = x.shape
+    ldq = (K + 15) // 16 * 16
+    q = torch.empty((M, ldq), dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty((M,), dtype=torch.float32, device=x.device)
+    check(lib().fvb_quantize_fp8_rows(ptr(x), c_int64(x.stride(0)), c_int(M), c_int(K), ptr(q), c_int64(ldq), _f32p(scale),
+                                      stream_ptr()))
+    return q[:, :K], scale
+
+
+class Fp8Weight:
+    """A linear weight w[N, K] held as e4m3 rows with one fp32 scale per output channel (w ~= q * scale[:, None])."""
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor):
+        if q.dtype != torch.float8_e4m3fn or q.dim() != 2 or q.stride(1) != 1 or q.stride(0) % 16 != 0:
+            raise FvbError("Fp8Weight.q must be float8_e4m3fn [N, K] with 16-byte-aligned rows")
+        if scale.dtype != torch.float32 or scale.shape != (q.shape[0],) or not scale.is_contiguous():
+            raise FvbError("Fp8Weight.scale must be fp32 [N] contiguous")
+        self.q, self.scale = q, scale
+
+    @classmethod
+    def quantize(cls, w: torch.Tensor) -> "Fp8Weight":
+        """bf16 [N, K] -> per-output-channel e4m3 (the same row quantisation as the activations)."""
+        return cls(*quantize_fp8_rows(w))
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    @property
+    def device(self):
+        return self.q.device
+
+    def dequantize(self) -> torch.Tensor:
+        """fp32 [N, K] values the GEMM multiplies with (q * scale)."""
+        return self.q.float() * self.scale[:, None]
+
+
+def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: torch.Tensor | None = None, epilogue: int = EPI_BIAS,
+               resid: torch.Tensor | None = None, gate: torch.Tensor | None = None,
+               out: torch.Tensor | None = None, gate_rows: int = 0) -> torch.Tensor:
+    """`linear` with e4m3 operands: x (bf16 [..., K]) is row-quantised here (fvb_quantize_fp8_rows), then
+    out = epilogue(bf16((q_x @ q_w.T) * s_x[m] * s_w[n] + bias)) by fvb_linear_fp8. Same epilogues, gate grouping and
+    output dtypes as `linear`."""
+    if not isinstance(w, Fp8Weight):
+        raise FvbError("linear_fp8 takes an Fp8Weight (see Fp8Weight.quantize)")
+    _require_cuda_bf16(x, "x")
+    K = x.shape[-1]
+    N = w.shape[0]
+    if w.shape[1] != K:
+        raise FvbError(f"x has K={K}, weight has K={w.shape[1]}")
+    x2 = x.reshape(-1, K)
+    if x2.stride(1) != 1 or x2.stride(0) % 8 != 0:
+        x2 = x2.contiguous()
+    M = x2.shape[0]
+    xq, xs = quantize_fp8_rows(x2)
+    out_dtype = torch.float32 if epilogue == EPI_RESID_GATE_F32 else torch.bfloat16
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=x.device)
+    o2 = out.reshape(M, N)
+    assert o2.dtype == out_dtype and o2.stride(1) == 1
+    r2 = None
+    if resid is not None:
+        _require_cuda_bf16(resid, "resid")
+        r2 = resid.reshape(M, N)
+        assert r2.stride(1) == 1
+    gate_stride = _check_grouped(gate, N, gate_rows, M, "gate")
+    if bias is not None:
+        _require_cuda_bf16(bias, "bias")
+        assert bias.is_contiguous() and bias.numel() == N
+    check(lib().fvb_linear_fp8(ptr(xq), c_int64(xq.stride(0)), _f32p(xs), ptr(w.q), c_int64(w.q.stride(0)), _f32p(w.scale),
+                               ptr(bias), ptr(o2), c_int64(o2.stride(0)), ptr(r2), c_int64(r2.stride(0) if r2 is not None else 0),
+                               _f32p(gate), c_int(gate_rows), c_int64(gate_stride), c_int(M), c_int(N), c_int(K),
+                               c_int(epilogue), stream_ptr()))
+    return out.reshape(*x.shape[:-1], N)
+
+
+def linear_any(x: torch.Tensor, w, *args, **kwargs) -> torch.Tensor:
+    """`linear_fp8` for an Fp8Weight, `linear` for a bf16 tensor."""
+    return (linear_fp8 if isinstance(w, Fp8Weight) else linear)(x, w, *args, **kwargs)
+
+
 def _check_grouped(t, D: int, rows: int, M: int, name: str) -> int:
     """Validate a per-row-group fp32 vector table ([D] when rows == 0, [G, D] otherwise); returns its group stride."""
     if t is None:

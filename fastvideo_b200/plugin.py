@@ -21,6 +21,9 @@ What install() registers, and the reference interface each piece stands behind:
   linear              @register_quantization_config("fvb200_bf16") Fvb200Bf16Config(QuantizationConfig) whose
                       get_quant_method returns Fvb200LinearMethod(LinearMethodBase)
                       (fastvideo/layers/quantization/__init__.py:13-45, base_config.py:17-140, layers/linear.py:80-156).
+  linear (FP8)        @register_quantization_config("fvb200_fp8") Fvb200Fp8Config: Fvb200Fp8LinearMethod loads the same
+                      bf16 weight, quantises it to e4m3 per output channel in process_weights_after_loading (the bf16
+                      parameter is replaced, not kept) and applies ops.linear_fp8 (activations quantised per token).
   custom ops          RMSNorm.forward_cuda (fastvideo/layers/layernorm.py:12-83) on fvb_rmsnorm_rope, and
                       CustomOp.dispatch_forward (fastvideo/layers/custom_op.py:53-57, hard-wired to forward_native) routed
                       to forward_cuda for the classes that got one.
@@ -42,6 +45,7 @@ from ._lib import FvbError
 
 DENSE_BACKEND_NAME = "FVB200_ATTN"
 QUANT_NAME = "fvb200_bf16"
+QUANT_NAME_FP8 = "fvb200_fp8"
 
 _state: types.SimpleNamespace | None = None
 
@@ -227,13 +231,47 @@ def _define():
         def get_quant_method(self, layer, prefix: str):
             return Fvb200LinearMethod() if isinstance(layer, LinearBase) else None
 
+    class Fvb200Fp8LinearMethod(Fvb200LinearMethod):
+        """Same bf16 weight parameter as Fvb200LinearMethod; after loading it becomes `weight` (float8_e4m3fn [N, K]) plus
+        `weight_scale` (fp32 [N]), and apply() runs fvb_quantize_fp8_rows + fvb_linear_fp8."""
+
+        def process_weights_after_loading(self, layer) -> None:
+            w = layer.weight
+            if not w.is_cuda:
+                raise FvbError("fvb200_fp8 quantises its weights on the GPU: load the model onto a CUDA device")
+            fw = ops.Fp8Weight.quantize(w.data.to(torch.bfloat16))
+            layer.weight = Parameter(fw.q, requires_grad=False)  # drops the bf16 parameter
+            layer.weight_scale = Parameter(fw.scale, requires_grad=False)
+
+        def apply(self, layer, x, bias=None):
+            if not x.is_cuda:
+                raise FvbError("fvb200_fp8 linear needs CUDA tensors (there is no CPU fallback)")
+            if layer.weight.dtype != torch.float8_e4m3fn:
+                raise FvbError("fvb200_fp8 linear: weights are not quantised (process_weights_after_loading did not run)")
+            if x.dtype != torch.bfloat16:
+                raise FvbError(f"fvb200_fp8 linear takes bf16 activations (got {x.dtype})")
+            w = ops.Fp8Weight(layer.weight, layer.weight_scale)
+            b = None if bias is None else bias.to(torch.bfloat16)
+            return ops.linear_fp8(x, w, b)
+
+    class Fvb200Fp8Config(Fvb200Bf16Config):
+        def get_name(self):
+            return QUANT_NAME_FP8
+
+        @classmethod
+        def get_min_capability(cls) -> int:
+            return 90  # e4m3 wgmma: sm_90a
+
+        def get_quant_method(self, layer, prefix: str):
+            return Fvb200Fp8LinearMethod() if isinstance(layer, LinearBase) else None
+
     ns.__dict__.update(
         Fvb200AttentionMetadata=Fvb200AttentionMetadata, Fvb200AttentionMetadataBuilder=Fvb200AttentionMetadataBuilder,
         Fvb200AttentionImpl=Fvb200AttentionImpl, Fvb200AttentionBackend=Fvb200AttentionBackend,
         Fvb200VideoSparseAttentionMetadata=Fvb200VideoSparseAttentionMetadata,
         Fvb200VideoSparseAttentionMetadataBuilder=Fvb200VideoSparseAttentionMetadataBuilder,
         Fvb200VideoSparseAttentionImpl=Fvb200VideoSparseAttentionImpl, Fvb200LinearMethod=Fvb200LinearMethod,
-        Fvb200Bf16Config=Fvb200Bf16Config)
+        Fvb200Bf16Config=Fvb200Bf16Config, Fvb200Fp8LinearMethod=Fvb200Fp8LinearMethod, Fvb200Fp8Config=Fvb200Fp8Config)
     return ns
 
 
@@ -350,6 +388,8 @@ def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, c
         from fastvideo.layers import quantization as Q
         if QUANT_NAME not in Q.QUANTIZATION_METHODS:
             Q.register_quantization_config(QUANT_NAME)(ns.Fvb200Bf16Config)
+        if QUANT_NAME_FP8 not in Q.QUANTIZATION_METHODS:
+            Q.register_quantization_config(QUANT_NAME_FP8)(ns.Fvb200Fp8Config)
 
     if custom_ops:
         from fastvideo.layers.custom_op import CustomOp
@@ -379,4 +419,5 @@ def uninstall() -> None:
     _state = None
 
 
-__all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "DENSE_BACKEND_NAME", "QUANT_NAME"]
+__all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "DENSE_BACKEND_NAME", "QUANT_NAME",
+           "QUANT_NAME_FP8"]

@@ -45,6 +45,10 @@ class WanDiTConfig:
     freq_dim: int = 256
     eps: float = 1e-6
     vsa: bool = False  # WanTransformerBlock_VSA (to_gate_compress present)
+    # Opt-in FP8: the six token-stream GEMMs of every block (FP8_LINEARS) run on e4m3 weights (per output channel) and
+    # e4m3 activations (per token) through ops.linear_fp8; those weights are quantised once at load and no bf16 copy is
+    # kept. The text-side K/V projections, the embedders, patch embedding and proj_out stay bf16.
+    fp8_linears: bool = False
 
     @property
     def head_dim(self) -> int:
@@ -99,6 +103,10 @@ def random_state_dict(cfg: WanDiTConfig, device="cuda", seed: int = 2029, dtype=
     return sd
 
 
+# WanBlock weights that multiply the token stream; with WanDiTConfig.fp8_linears they are ops.Fp8Weight
+FP8_LINEARS = ("w_qkv", "w_o", "w_q2", "w_o2", "w_1", "w_2")
+
+
 class WanBlock:
     """Weights of one transformer block in the layout the kernels want."""
 
@@ -131,6 +139,9 @@ class WanBlock:
         self.w_1, self.b_1 = bf(g("ffn.fc_in.weight")), bf(g("ffn.fc_in.bias"))
         self.w_2, self.b_2 = bf(g("ffn.fc_out.weight")), bf(g("ffn.fc_out.bias"))
         self.scale_shift_table = g("scale_shift_table")  # dtype as loaded: the modulation sum happens in torch
+        if cfg.fp8_linears:
+            for n in FP8_LINEARS:  # replacing the attribute drops the block's bf16 copy
+                setattr(self, n, ops.Fp8Weight.quantize(getattr(self, n)))
 
 
 @dataclass
@@ -176,7 +187,7 @@ def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: Wan
     S, D = n2.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
     hd = lambda t: t.unflatten(1, (H, d)).unsqueeze(0)
-    q2 = ops.linear(n2, blk.w_q2, blk.b_q2)
+    q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
     ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
     img = None
     if blk.w_kv_img is not None:
@@ -203,7 +214,7 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
 
     # 1. self-attention (wanvideo.py:393-415)
     n1 = ops.layernorm_modulate(x, scale_msa, shift_msa, eps=cfg.eps)
-    qkv = ops.linear(n1, blk.w_qkv, blk.b_qkv)  # [S, 3D or 4D]
+    qkv = ops.linear_any(n1, blk.w_qkv, blk.b_qkv)  # [S, 3D or 4D]
     ops.rmsnorm_rope_(qkv[:, :D], blk.norm_q, qkv[:, D:2 * D], blk.norm_k, lay.cos, lay.sin, lay.rope_row, head_dim=d,
                       eps=cfg.eps)
     q = qkv[:, :D].unflatten(1, (H, d)).unsqueeze(0)
@@ -217,17 +228,17 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
         a = ops.attention(q, k, v, softmax_scale=d ** -0.5)
     a = a.reshape(S, D)
     # to_out + gated residual in fp32, then LN(affine) and the bf16 residual stream (wanvideo.py:415-421)
-    r32 = ops.linear(a, blk.w_o, blk.b_o, ops.EPI_RESID_GATE_F32, resid=x, gate=gate_msa)
+    r32 = ops.linear_any(a, blk.w_o, blk.b_o, ops.EPI_RESID_GATE_F32, resid=x, gate=gate_msa)
     n2, x = ops.layernorm_modulate(r32, None, None, blk.norm2_w, blk.norm2_b, eps=cfg.eps, want_hidden=True)
 
     # 2. cross-attention (wanvideo.py:188-222, 424-427)
     a2 = cross_attention(n2, blk, ctx, cfg)
-    x = ops.linear(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
+    x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
     n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps)
 
     # 3. feed-forward (wanvideo.py:430-432)
-    f = ops.linear(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-    x = ops.linear(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
+    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+    x = ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
     return x
 
 
@@ -260,7 +271,7 @@ class WanDiT:
     @classmethod
     def random(cls, cfg: WanDiTConfig, device="cuda", seed: int = 2029) -> "WanDiT":
         """Synthetic random-init model of the given architecture, built layer by layer so that peak memory stays
-        at one copy of the weights (30 GB for a 14B expert)."""
+        at one copy of the weights (30 GB for a 14B expert in bf16; with fp8_linears the block weights take half)."""
         blocks = []
         for i in range(cfg.num_layers):
             one = WanDiTConfig(**{**cfg.__dict__, "num_layers": 1})

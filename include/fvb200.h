@@ -80,6 +80,33 @@ int fvb_linear_bf16_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_
                        int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M, int N, int K,
                        int epilogue, void* stream);
 
+/* --------------------------------------------------------------------------------------------
+ * FP8 (e4m3) linear layers: row-quantised activations x per-output-channel-quantised weights
+ * Stands behind FastVideo's FP8 linear (fastvideo/layers/fp8linear.py, fastvideo/layers/quantization/) with this
+ * library's own arithmetic, below.
+ *
+ * fvb_quantize_fp8_rows: x bf16 [M, K] (row stride ldx, a multiple of 8: 16-byte rows; K a multiple of 8)
+ *   -> q e4m3 [M, K] (one byte per element, row stride ldq, a multiple of 8) and scale fp32 [M]:
+ *   amax = max_k |x[r, k]| (fp32, exact);
+ *   amax == 0: scale[r] = 1, q[r, :] = 0;
+ *   else inv = 448.0f / amax, q[r, k] = e4m3_satfinite_rn(x[r, k] * inv), scale[r] = amax / 448.0f
+ *   (IEEE round-to-nearest division and multiplication; e4m3_satfinite_rn = __nv_cvt_float_to_fp8(v, __NV_SATFINITE,
+ *   __NV_E4M3)). Used for activations (one scale per token) and for weights w[N, K] (one scale per output channel).
+ *
+ * fvb_linear_fp8: xq e4m3 [M, K] ld=ldx with x_scale fp32 [M]; wq e4m3 [N, K] ld=ldw with w_scale fp32 [N]:
+ *   acc[m, n] = sum_k xq[m, k] * wq[n, k]                (fp32: partial sums leave the tensor core every 128 k)
+ *   y = bf16(((acc * x_scale[m]) * w_scale[n]) + bias[n])  (fp32 round-to-nearest, in that order; bias may be NULL)
+ *   then the epilogue exactly as in fvb_linear_bf16: FVB_EPI_BIAS, BIAS_GELU_TANH, RESID_GATE_F32, RESID_GATE_BF16,
+ *   RESID_GATE_BF16R, RESID_BF16, with the same gate / gate_rows grouping.
+ *   ldx, ldw multiples of 16 (16-byte rows); ldo, ldr multiples of 8; N a multiple of 8 when bias / residual are used.
+ *   K tails (K not a multiple of 128) are zero-filled on load.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_quantize_fp8_rows(const void* x, int64_t ldx, int M, int K, void* q, int64_t ldq, float* scale, void* stream);
+
+int fvb_linear_fp8(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw, const float* w_scale,
+                   const void* bias, void* out, int64_t ldo, const void* resid, int64_t ldr, const float* gate, int gate_rows,
+                   int64_t gate_stride, int M, int N, int K, int epilogue, void* stream);
+
 /* Batched C[i] = bf16(A[i] @ B[i]^T), optionally followed by out = bf16(float(C) / div) (div = 0 or 1: none).
  * A[i]: [M, K] ld=lda, B[i]: [N, K] ld=ldb, out[i]: [M, N] ld=ldo; batch strides in elements (multiples of 8).
  * Replaces the block-level matmuls of video_sparse_attn's compression branch
