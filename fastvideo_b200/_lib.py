@@ -29,6 +29,7 @@ def lib() -> ctypes.CDLL:
         _lib.fvb_last_error.restype = c_char_p
         _lib.fvb_abi_version.restype = c_int
         _lib.fvb_attention_blocklist_workspace_bytes.restype = c_int64
+        _lib.fvb_attention_8bit_workspace_bytes.restype = c_int64
     return _lib
 
 

@@ -64,6 +64,16 @@ class B200AttentionImpl:
         return ops.attention(query, key, value, softmax_scale=self.softmax_scale)
 
 
+class B200Attention8bitImpl(B200AttentionImpl):
+    """B200AttentionImpl on the 8-bit attention (INT8 Q K^T, FP8 P V): q, k, v are quantised per call
+    (ops.quantize_attention_8bit), then ops.attention_8bit."""
+
+    def forward(self, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, attn_metadata=None) -> torch.Tensor:
+        if attn_metadata is not None and getattr(attn_metadata, "attn_mask", None) is not None:
+            raise NotImplementedError("dense boolean masks: use block lists (block_sparse_attn_from_indices / STA)")
+        return ops.attention_8bit(ops.quantize_attention_8bit(query, key, value), self.softmax_scale)
+
+
 class B200AttentionBackend:
     accept_output_buffer: bool = True
 

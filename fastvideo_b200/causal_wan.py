@@ -265,23 +265,25 @@ def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb
     return ops.linear(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=tpf)
 
 
-def _require_bf16_linears(cfg: WanDiTConfig) -> None:
+def _require_bf16_model(cfg: WanDiTConfig) -> None:
     if cfg.fp8_linears:
         raise ops.FvbError("the causal rollout runs bf16 linears only: build the model with fp8_linears=False")
+    if cfg.attention_8bit:
+        raise ops.FvbError("the causal rollout runs bf16 attention only: build the model with attention_8bit=False")
 
 
 class CausalWanDiT(WanDiT):
     """CausalWanTransformer3DModel._forward_inference on libfvb200 (batch 1 per call, like the rollout stage)."""
 
     def __init__(self, cfg: WanDiTConfig, state_dict: dict, ccfg: CausalConfig, blocks: list | None = None):
-        _require_bf16_linears(cfg)
+        _require_bf16_model(cfg)
         super().__init__(cfg, state_dict, blocks)
         self.ccfg = ccfg
         self._rope: dict = {}
 
     @classmethod
     def random(cls, cfg: WanDiTConfig, ccfg: CausalConfig, device="cuda", seed: int = 2029) -> "CausalWanDiT":
-        _require_bf16_linears(cfg)
+        _require_bf16_model(cfg)
         base = WanDiT.random(cfg, device, seed)
         m = cls.__new__(cls)
         m.__dict__.update(base.__dict__)
@@ -378,7 +380,7 @@ class SPCausalWanDiT:
 
     def __init__(self, model: CausalWanDiT, rank: int, world: int, group=None):
         import torch.distributed as dist
-        _require_bf16_linears(model.cfg)
+        _require_bf16_model(model.cfg)
         self.m, self.rank, self.world = model, rank, world
         self.group = group or dist.group.WORLD
         if model.cfg.num_attention_heads % world:

@@ -156,6 +156,9 @@ class SPWanDiT:
         if model.cfg.fp8_linears:
             from ._lib import FvbError
             raise FvbError("sequence parallelism runs bf16 linears only: build the model with fp8_linears=False")
+        if model.cfg.attention_8bit:
+            from ._lib import FvbError
+            raise FvbError("sequence parallelism runs bf16 attention only: build the model with attention_8bit=False")
         self.m = model
         self.rank, self.world, self.group = rank, world, group
         self._plans: dict = {}

@@ -346,6 +346,101 @@ def attention_blocklist(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q2k_i
     return (out, lse) if return_lse else out
 
 
+class Attn8bitInputs:
+    """Operands of the 8-bit attention, from quantize_attention_8bit (layouts and arithmetic in include/fvb200.h,
+    fvb_attention_8bit_quantize): q8 / k8 int8 [B, H, S, 128] with q_scale / k_scale fp32 [B, H, S]; vt8 float8_e4m3fn
+    [B, H, nkb, 128, 64] (V transposed per 64-key block, key slots permuted) with v_scale fp32 [B, H, 128]; k_mean fp32
+    [B, H, 128] (the mean key subtracted before quantising K). kv_off / kv_len / nkb: the key blocks vt8 is laid out by."""
+
+    def __init__(self, q8, q_scale, k8, k_scale, k_mean, vt8, v_scale, kv_off, kv_len, nkb):
+        self.q8, self.q_scale, self.k8, self.k_scale, self.k_mean = q8, q_scale, k8, k_scale, k_mean
+        self.vt8, self.v_scale = vt8, v_scale
+        self.kv_off, self.kv_len, self.nkb = kv_off, kv_len, nkb
+
+    @property
+    def shape(self):
+        """(B, H, Sq, Skv)"""
+        B, H, Sq, _ = self.q8.shape
+        return B, H, Sq, self.k8.shape[2]
+
+
+def _check_i32(t, name: str, n: int) -> None:
+    if t is not None and (t.dtype != torch.int32 or not t.is_cuda or not t.is_contiguous() or t.numel() < n):
+        raise FvbError(f"{name} must be a contiguous int32 CUDA tensor of at least {n} elements")
+
+
+def quantize_attention_8bit(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, kv_off=None, kv_len=None,
+                            nkb: int | None = None) -> Attn8bitInputs:
+    """fvb_attention_8bit_quantize. q: [B, Sq, H, 128], k/v: [B, Skv, H, 128] bf16 views (any (b, s, h) strides that are
+    multiples of 8, e.g. the column slices of a fused QKV buffer). kv_off int32 [nkb + 1] / kv_len int32 [nkb] define the key
+    blocks (default: 64-key blocks, nkb = ceil(Skv / 64))."""
+    for n, t in (("q", q), ("k", k), ("v", v)):
+        _require_cuda_bf16(t, n)
+    B, Sq, H, d = q.shape
+    Skv = k.shape[1]
+    if d != 128 or k.shape != (B, Skv, H, d) or v.shape != k.shape:
+        raise FvbError("q, k, v must be [B, S, H, 128] with matching B, H and key counts")
+    if kv_off is None:
+        nkb = (Skv + 63) // 64 if nkb is None else nkb
+    elif nkb is None:
+        nkb = kv_off.numel() - 1
+    _check_i32(kv_off, "kv_off", nkb + 1)
+    _check_i32(kv_len, "kv_len", nkb)
+    dev = q.device
+    q8 = torch.empty((B, H, Sq, d), dtype=torch.int8, device=dev)
+    k8 = torch.empty((B, H, Skv, d), dtype=torch.int8, device=dev)
+    q_scale = torch.empty((B, H, Sq), dtype=torch.float32, device=dev)
+    k_scale = torch.empty((B, H, Skv), dtype=torch.float32, device=dev)
+    k_mean = torch.empty((B, H, d), dtype=torch.float32, device=dev)
+    vt8 = torch.empty((B, H, nkb, d, 64), dtype=torch.float8_e4m3fn, device=dev)
+    v_scale = torch.empty((B, H, d), dtype=torch.float32, device=dev)
+    ws = _workspace(int(lib().fvb_attention_8bit_workspace_bytes(c_int(B), c_int(H), c_int(Skv))), dev)
+    check(lib().fvb_attention_8bit_quantize(ptr(q), ptr(k), ptr(v), _bsh_strides(q), _bsh_strides(k), _bsh_strides(v), c_int(B),
+                                            c_int(H), c_int(Sq), c_int(Skv), c_int(d), _i32p(kv_off), _i32p(kv_len), c_int(nkb),
+                                            ptr(q8), _f32p(q_scale), ptr(k8), _f32p(k_scale), _f32p(k_mean), ptr(vt8),
+                                            _f32p(v_scale), ptr(ws), c_int64(ws.numel()), stream_ptr()))
+    return Attn8bitInputs(q8, q_scale, k8, k_scale, k_mean, vt8, v_scale, kv_off, kv_len, nkb)
+
+
+def attention_8bit(inputs: Attn8bitInputs, softmax_scale: float | None = None, q2k_idx: torch.Tensor | None = None,
+                   q2k_num: torch.Tensor | None = None, q_off=None, q_len=None, out: torch.Tensor | None = None) -> torch.Tensor:
+    """fvb_attention_8bit_fwd on quantize_attention_8bit's output -> bf16 [B, Sq, H, 128] (or into `out`, a BSHD view).
+    Dense keys without q2k_idx / q2k_num; otherwise per-q-block lists q2k_idx int32 [B or 1, H or 1, nqb, cap] (ascending,
+    first q2k_num[..] valid) with q blocks q_off / q_len, as in attention_blocklist. The key blocks are the quantiser's."""
+    if not isinstance(inputs, Attn8bitInputs):
+        raise FvbError("attention_8bit takes the Attn8bitInputs of quantize_attention_8bit")
+    B, H, Sq, Skv = inputs.shape
+    d = 128
+    if softmax_scale is None:
+        softmax_scale = d ** -0.5
+    if out is None:
+        alloc = torch.zeros if (q2k_idx is not None and q_off is None and q_len is not None) else torch.empty
+        out = alloc((B, Sq, H, d), dtype=torch.bfloat16, device=inputs.q8.device)
+    _require_cuda_bf16(out, "out")
+    if out.shape != (B, Sq, H, d):
+        raise FvbError(f"out must be [{B}, {Sq}, {H}, {d}]")
+    if (q2k_idx is None) != (q2k_num is None):
+        raise FvbError("q2k_idx and q2k_num go together")
+    nqb = cap = stride_b = stride_h = 0
+    if q2k_idx is not None:
+        if q2k_idx.dtype != torch.int32 or q2k_idx.dim() != 4 or not q2k_idx.is_contiguous():
+            raise FvbError("q2k_idx must be contiguous int32 [B or 1, H or 1, nqb, cap]")
+        ib, ih, nqb, cap = q2k_idx.shape
+        if q2k_num.dtype != torch.int32 or not q2k_num.is_contiguous() or q2k_num.shape != (ib, ih, nqb):
+            raise FvbError("q2k_num must be contiguous int32 [B or 1, H or 1, nqb]")
+        stride_h = 0 if ih == 1 else nqb
+        stride_b = 0 if ib == 1 else ih * nqb
+        _check_i32(q_off, "q_off", nqb + 1)
+        _check_i32(q_len, "q_len", nqb)
+    check(lib().fvb_attention_8bit_fwd(ptr(inputs.q8), _f32p(inputs.q_scale), ptr(inputs.k8), _f32p(inputs.k_scale),
+                                       ptr(inputs.vt8), _f32p(inputs.v_scale), ptr(out), None, _bsh_strides(out), c_int(B),
+                                       c_int(H), c_int(Sq), c_int(Skv), c_int(d), c_float(softmax_scale), None, _i32p(q2k_idx),
+                                       _i32p(q2k_num), c_int64(stride_b), c_int64(stride_h), c_int(cap), _i32p(q_off),
+                                       _i32p(q_len), c_int(nqb), _i32p(inputs.kv_off), _i32p(inputs.kv_len),
+                                       c_int(inputs.nkb), stream_ptr()))
+    return out
+
+
 def attention_blocklist_bwd(q, k, v, o, lse, dO, q2k_idx, q2k_num, k2q_idx, k2q_num, kv_len=None, softmax_scale=None):
     """Backward of attention_blocklist in the padded layout. q/k/v/o/dO: [B, S, H, 128] views; lse fp32 [B, H, Sq] contiguous;
     index tensors int32 [B or 1, H or 1, n, cap] / [.., n]. Returns (dq, dk, dv) with q's / k's / v's shapes (BSHD views)."""

@@ -12,6 +12,9 @@ What install() registers, and the reference interface each piece stands behind:
                       requests for FLASH_ATTN / TORCH_SDPA / "no preference" resolve to it; its get_name() is the distinct
                       "FVB200_ATTN", added to AttentionBackendEnum (fastvideo/platforms/interface.py:13-27) so that
                       `backend_name_to_enum(get_name())` (fastvideo/attention/layer.py:78) resolves.
+  attention (8-bit)   Fvb200Attention8bitBackend / Impl: the same contract on the 8-bit attention (INT8 Q K^T, FP8 P V,
+                      ops.attention_8bit), under its own enum member "FVB200_ATTN_8BIT". Only an explicit selection of that
+                      name resolves to it (same bf16 / head_size 128 / sm_90 rules); the reference's SAGE_ATTN is untouched.
   attention (VSA)     Fvb200VideoSparseAttentionImpl / MetadataBuilder / Metadata subclass the classes in
                       fastvideo/attention/backends/video_sparse_attn.py:115-342 and are returned by the reference's OWN
                       `VideoSparseAttentionBackend.get_impl_cls / get_builder_cls / get_metadata_cls`: Wan picks
@@ -44,6 +47,7 @@ from . import ops
 from ._lib import FvbError
 
 DENSE_BACKEND_NAME = "FVB200_ATTN"
+DENSE_8BIT_BACKEND_NAME = "FVB200_ATTN_8BIT"
 QUANT_NAME = "fvb200_bf16"
 QUANT_NAME_FP8 = "fvb200_fp8"
 
@@ -135,6 +139,23 @@ def _define():
         @staticmethod
         def get_builder_cls():
             return Fvb200AttentionMetadataBuilder
+
+    class Fvb200Attention8bitImpl(Fvb200AttentionImpl):
+        """Fvb200AttentionImpl on the 8-bit attention (attention.B200Attention8bitImpl)."""
+
+        def __init__(self, num_heads: int, head_size: int, softmax_scale: float | None = None, causal: bool = False,
+                     num_kv_heads: int | None = None, prefix: str = "", **extra_impl_args) -> None:
+            self._impl = _mirror.B200Attention8bitImpl(num_heads, head_size, causal=causal, softmax_scale=softmax_scale,
+                                                       num_kv_heads=num_kv_heads, prefix=prefix)
+
+    class Fvb200Attention8bitBackend(Fvb200AttentionBackend):
+        @staticmethod
+        def get_name() -> str:
+            return DENSE_8BIT_BACKEND_NAME
+
+        @staticmethod
+        def get_impl_cls():
+            return Fvb200Attention8bitImpl
 
     # ------------------------------------------------------------------ Video Sparse Attention
     @dataclass
@@ -268,6 +289,7 @@ def _define():
     ns.__dict__.update(
         Fvb200AttentionMetadata=Fvb200AttentionMetadata, Fvb200AttentionMetadataBuilder=Fvb200AttentionMetadataBuilder,
         Fvb200AttentionImpl=Fvb200AttentionImpl, Fvb200AttentionBackend=Fvb200AttentionBackend,
+        Fvb200Attention8bitImpl=Fvb200Attention8bitImpl, Fvb200Attention8bitBackend=Fvb200Attention8bitBackend,
         Fvb200VideoSparseAttentionMetadata=Fvb200VideoSparseAttentionMetadata,
         Fvb200VideoSparseAttentionMetadataBuilder=Fvb200VideoSparseAttentionMetadataBuilder,
         Fvb200VideoSparseAttentionImpl=Fvb200VideoSparseAttentionImpl, Fvb200LinearMethod=Fvb200LinearMethod,
@@ -322,6 +344,24 @@ def device_supported() -> bool:
     return torch.cuda.is_available() and tuple(torch.cuda.get_device_capability()) == (9, 0)
 
 
+def route_dense(selected: str | None, head_size: int, dtype, force: bool = False) -> str | None:
+    """Which dense backend of this package serves a request for the AttentionBackendEnum member named `selected` (None: no
+    preference): the qualified class name, or None to leave the request to the platform. bf16, head_size 128 and a
+    compute capability 9.0 device (or `force`) are required. FVB200_ATTN_8BIT is served only when selected by name; the
+    bf16 backend also takes FLASH_ATTN / TORCH_SDPA / no-preference requests unless FVB200_ATTENTION=0."""
+    ok = (force or device_supported()) and head_size == 128 and dtype == torch.bfloat16
+    if selected == DENSE_8BIT_BACKEND_NAME:
+        if not ok:
+            raise ValueError(f"{DENSE_8BIT_BACKEND_NAME} supports bf16 with head_size 128 on sm_90 only")
+        return f"{__name__}.Fvb200Attention8bitBackend"
+    if (ok and selected in (None, "FLASH_ATTN", "TORCH_SDPA", DENSE_BACKEND_NAME)
+            and os.environ.get("FVB200_ATTENTION", "1") != "0"):
+        return f"{__name__}.Fvb200AttentionBackend"
+    if selected == DENSE_BACKEND_NAME:
+        raise ValueError(f"{DENSE_BACKEND_NAME} supports bf16 with head_size 128 on sm_90 only")
+    return None
+
+
 def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, custom_ops: bool = True,
             force: bool | None = None):
     """Registers everything (idempotent). `force=True` routes the dense backend even when the current device is not
@@ -355,20 +395,15 @@ def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, c
 
     if dense:
         _extend_enum(AttentionBackendEnum, DENSE_BACKEND_NAME)
+        _extend_enum(AttentionBackendEnum, DENSE_8BIT_BACKEND_NAME)
         plat_cls = type(current_platform) if not isinstance(current_platform, type) else current_platform
         orig = plat_cls.__dict__.get("get_attn_backend_cls") or getattr(plat_cls, "get_attn_backend_cls")
         orig_fn = orig.__func__ if isinstance(orig, classmethod) else orig
-        routed = (None, AttentionBackendEnum.FLASH_ATTN, AttentionBackendEnum.TORCH_SDPA,
-                  AttentionBackendEnum[DENSE_BACKEND_NAME])
 
         def get_attn_backend_cls(cls, selected_backend, head_size, dtype):
-            on_device = force or device_supported()
-            if (on_device and selected_backend in routed and head_size == 128 and dtype == torch.bfloat16
-                    and os.environ.get("FVB200_ATTENTION", "1") != "0"):
-                return f"{__name__}.Fvb200AttentionBackend"
-            if selected_backend is AttentionBackendEnum[DENSE_BACKEND_NAME]:
-                raise ValueError(f"{DENSE_BACKEND_NAME} supports bf16 with head_size 128 on sm_90 only")
-            return orig_fn(cls, selected_backend, head_size, dtype)
+            name = None if selected_backend is None else selected_backend.name
+            routed = route_dense(name, head_size, dtype, force)
+            return routed if routed is not None else orig_fn(cls, selected_backend, head_size, dtype)
 
         patch(plat_cls, "get_attn_backend_cls", classmethod(get_attn_backend_cls))
         try:  # the resolution is functools-cached on its arguments (attention/selector.py:239)
@@ -419,5 +454,5 @@ def uninstall() -> None:
     _state = None
 
 
-__all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "DENSE_BACKEND_NAME", "QUANT_NAME",
-           "QUANT_NAME_FP8"]
+__all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "route_dense", "DENSE_BACKEND_NAME",
+           "DENSE_8BIT_BACKEND_NAME", "QUANT_NAME", "QUANT_NAME_FP8"]

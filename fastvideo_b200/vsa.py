@@ -28,9 +28,11 @@ SPARSE_KERNEL = os.environ.get("FVB_VSA_KERNEL", "ws")
 
 
 def video_sparse_attn_bshd(q, k, v, variable_block_sizes, topk: int, gate=None, block_off=None, row_block=None,
-                           out=None, return_aux: bool = False, out_segments=None):
+                           out=None, return_aux: bool = False, out_segments=None, attn_8bit: bool = False):
     """q/k/v/gate: [B, S, H, 128] bf16 views (strided ok). variable_block_sizes: int32 [nblk] on device.
     block_off: int32 [nblk+1] for the compact layout, None for the padded one.
+    attn_8bit: the sparse branch runs the 8-bit attention (ops.quantize_attention_8bit once, then ops.attention_8bit on the
+    per-q-block lists); the compression branch stays bf16.
     out_segments = (int64 device table of P base addresses, rows per segment, (b, s, h) element strides): the result rows
     are stored segment by segment at those addresses (sequence-parallel return path: peer memory) instead of `out`."""
     B, S, H, d = q.shape
@@ -44,7 +46,14 @@ def video_sparse_attn_bshd(q, k, v, variable_block_sizes, topk: int, gate=None, 
     scores = ops.gemm_batched(q_c.view(B * H, nblk, d), k_c.view(B * H, nblk, d), div=math.sqrt(d))  # [BH, nq, nk]
     attn = ops.softmax_rows(scores)
     out_c = ops.gemm_batched(attn, v_ct.reshape(B * H, d, -1)).contiguous().view(B, H, nblk, d)
-    if SPARSE_KERNEL == "ws":
+    if attn_8bit:
+        q2k_idx, q2k_num, mask = ops.topk_index(scores, topk, want_mask=return_aux)
+        q2k_idx, q2k_num = q2k_idx.view(B, H, nblk, nblk), q2k_num.view(B, H, nblk)
+        if mask is not None:
+            mask = mask.view(B, H, nblk, nblk)
+        qin = ops.quantize_attention_8bit(q, k, v, kv_off=block_off, kv_len=vbs, nkb=nblk)
+        out_s = ops.attention_8bit(qin, d ** -0.5, q2k_idx, q2k_num, q_off=block_off, q_len=vbs)
+    elif SPARSE_KERNEL == "ws":
         # block map and index lists in one pass over the scores (fvb_topk_index); the boolean map only when the caller asks
         q2k_idx, q2k_num, mask = ops.topk_index(scores, topk, want_mask=return_aux)
         q2k_idx, q2k_num = q2k_idx.view(B, H, nblk, nblk), q2k_num.view(B, H, nblk)

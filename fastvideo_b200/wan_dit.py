@@ -49,6 +49,9 @@ class WanDiTConfig:
     # e4m3 activations (per token) through ops.linear_fp8; those weights are quantised once at load and no bf16 copy is
     # kept. The text-side K/V projections, the embedders, patch embedding and proj_out stay bf16.
     fp8_linears: bool = False
+    # Opt-in 8-bit self-attention (INT8 Q K^T, FP8 P V; ops.quantize_attention_8bit + ops.attention_8bit), dense and the VSA
+    # sparse branch. Cross-attention and the VSA compression branch stay bf16. Independent of fp8_linears.
+    attention_8bit: bool = False
 
     @property
     def head_dim(self) -> int:
@@ -223,7 +226,9 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
     if cfg.vsa:
         gate = qkv[:, 3 * D:4 * D].unflatten(1, (H, d)).unsqueeze(0)
         a = vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=gate, block_off=lay.block_off,
-                                       row_block=lay.row_block)
+                                       row_block=lay.row_block, attn_8bit=cfg.attention_8bit)
+    elif cfg.attention_8bit:
+        a = ops.attention_8bit(ops.quantize_attention_8bit(q, k, v), d ** -0.5)
     else:
         a = ops.attention(q, k, v, softmax_scale=d ** -0.5)
     a = a.reshape(S, D)

@@ -210,6 +210,55 @@ int fvb_attention_blocklist_fwd(const void* q, const void* k, const void* v, voi
  * compatibility only: the sm_90a kernel merges the two lists of a CTA while it walks them and uses no workspace. */
 int64_t fvb_attention_blocklist_workspace_bytes(int index_rows, int nqb, int cap);
 
+/* --------------------------------------------------------------------------------------------
+ * 8-bit attention forward (opt-in; INT8 Q K^T, FP8 e4m3 P V), head_dim 128, bf16 in and out. The SageAttention2 scheme,
+ * a quantised alternative to FastVideo's SAGE_ATTN backends (fastvideo/attention/backends/sage_attn.py) with this
+ * library's own arithmetic, below. Per batch b and head h, every op fp32 round-to-nearest unless stated:
+ *   K smoothing: k_mean[c] = (sum over all Skv keys of float(k[s, c])) / Skv -- per-256-key chunk sums in key order, then
+ *     the chunk sums in chunk order (no atomics: the same result on every run); k'[s, c] = float(k[s, c]) - k_mean[c]. This
+ *     adds q . k_mean to every logit of a row, so the softmax does not change.
+ *   Q and K' to int8, one scale per (token, head) row of 128: amax = max |x|; amax == 0: scale = 1, row = 0; else
+ *     inv = 127 / amax, x8 = clamp(rint(x * inv), -127, 127), scale = amax / 127.
+ *   V to e4m3, one scale per (head, channel) over all Skv keys: amax = max_s |v[s, c]|; amax == 0: v_scale = 1, v8 = 0; else
+ *     v8 = e4m3_satfinite_rn(v * (448 / amax)), v_scale = amax / 448.
+ *   Logits: x = ((float(acc) * q_scale[m]) * k_scale[n]) * (softmax_scale * log2 e), acc the exact integer Q8 . K8 (s32);
+ *     keys past a block's valid length are -inf.
+ *   Online softmax over the 64-key tiles in the kernel's walk order: m = running max, p = exp2(x - m) (ex2.approx),
+ *     l = l * alpha + sum of the unquantised p, alpha = exp2(m_old - m); p8 = e4m3_rn(p * 448).
+ *   P V in two levels: T = sum over the tile's 64 key slots of p8 * v8 (tensor-core accumulation, into a fresh register set),
+ *     then O = (O * alpha) + T (fp32).
+ *   Output: o[m, c] = bf16((O[m, c] * v_scale[c]) * (1 / (448 * l[m]))); a row with no keys gives zeros. No LSE is written.
+ *
+ * fvb_attention_8bit_quantize: q [B, Sq, H, 128], k / v [B, Skv, H, 128] bf16 through (b, s, h) element strides (multiples of
+ * 8; the views of a fused QKV buffer work in place) -> q8 int8 [B, H, Sq, 128], q_scale fp32 [B, H, Sq], k8 int8
+ * [B, H, Skv, 128], k_scale fp32 [B, H, Skv], k_mean fp32 [B, H, 128], v_scale fp32 [B, H, 128] and
+ *   vt8 e4m3 [B][H][nkb][128 channels][64 key slots]: key block kb, channel c, slot j holds v8 of key
+ *     16 (j >> 4) + 2 ((j & 15) >> 2) + (j & 1) + 8 ((j >> 1) & 1) of the block, i.e. slot j of each 16-key group holds key
+ *     2 (j >> 2) + (j & 1) + 8 ((j >> 1) & 1) of that group; slots of keys past the block's valid length are 0.
+ *   This order lets P go from the S accumulator registers straight into the A-operand registers of the e4m3 wgmma.
+ *   Key blocks as in fvb_attention_blocklist_fwd: kv_off (optional, [nkb + 1]) the first row of each block, kv_len (optional,
+ *   [nkb]) the valid keys; without kv_off, block i is keys [64 i, 64 i + 64) and nkb must be ceil(Skv / 64).
+ *   workspace: device memory of fvb_attention_8bit_workspace_bytes(B, H, Skv) bytes, 256-byte aligned.
+ *
+ * fvb_attention_8bit_fwd: the attention above on the quantiser's outputs (same B, H, Sq, Skv, key blocks kv_off / kv_len /
+ * nkb). o bf16 through (b, s, h) element strides. Dense keys (every key block) with q2k_idx == q2k_num == NULL; otherwise
+ * per-q-block lists with the format, q_off / q_len, masking and empty-row rules of fvb_attention_blocklist_fwd. lse must be
+ * NULL (FVB_ERR_INVALID_ARG otherwise); the pair-schedule (STA) mode, sched != NULL, returns FVB_ERR_UNSUPPORTED.
+ * -------------------------------------------------------------------------------------------- */
+int64_t fvb_attention_8bit_workspace_bytes(int B, int H, int Skv);
+
+int fvb_attention_8bit_quantize(const void* q, const void* k, const void* v, const int64_t* q_strides, const int64_t* k_strides,
+                                const int64_t* v_strides, int B, int H, int Sq, int Skv, int head_dim, const int32_t* kv_off,
+                                const int32_t* kv_len, int nkb, void* q8, float* q_scale, void* k8, float* k_scale,
+                                float* k_mean, void* vt8, float* v_scale, void* workspace, int64_t workspace_bytes,
+                                void* stream);
+
+int fvb_attention_8bit_fwd(const void* q8, const float* q_scale, const void* k8, const float* k_scale, const void* vt8,
+                           const float* v_scale, void* o, float* lse, const int64_t* o_strides, int B, int H, int Sq, int Skv,
+                           int head_dim, float softmax_scale, const int32_t* sched, const int32_t* q2k_idx,
+                           const int32_t* q2k_num, int64_t idx_stride_b, int64_t idx_stride_h, int cap, const int32_t* q_off,
+                           const int32_t* q_len, int nqb, const int32_t* kv_off, const int32_t* kv_len, int nkb, void* stream);
+
 /* Backward of fvb_attention_blocklist_fwd in the padded layout (block i = rows [64 i, 64 i + 64)): dq, dk, dv from q, k, v, o,
  * the forward's LSE (log2 domain) and dO. q2k_* as in the forward; k2q_idx int32 [.., nkb, capk] / k2q_num [.., nkb] list,
  * ascending, the q blocks that selected each kv block (the inverse lists, triton_kernels/index.py:147-250 invert_indices);
