@@ -1,19 +1,24 @@
 // vae_ops.cu -- bandwidth-bound pieces of the Wan VAE decoder on channels-last frames [pixels][C]:
 //   fvb_rmsnorm_silu_cl   WanRMS_norm (F.normalize * sqrt(C) * gamma) [+ SiLU]   (wanvae.py:210-233, 414-446)
+//   fvb_rmsnorm_silu_cl_e4m3  the same, written as e4m3 with a static per-tensor scale (input of an FP8 convolution)
 //   fvb_upsample2x_cl     nearest-exact 2x spatial upsample                        (wanvae.py:236-248, 272-281)
 //   fvb_transpose_bf16    [R, C] -> [C, R]                                         (V^T for the mid-block attention)
 //   fvb_softmax_rows_f32  fp32 scores -> bf16 probabilities, rows of any length    (SDPA of WanAttentionBlock, wanvae.py:495)
 //   fvb_clamp_to_nchw     channels-last bf16 -> clamp(-1,1) fp32 NCTHW             (wanvae.py:1210-1211)
+#include <cuda_fp8.h>
+
 #include "fvb_host.cuh"
 #include "fvb_ptx.cuh"
 
 namespace fvb {
 
 // one warp per pixel; y = x / max(||x||_2, 1e-12) * sqrt(C) * gamma (+ beta), optional SiLU; fp32 math, bf16 out
+// E4M3: out holds e4m3 bytes, q = e4m3_satfinite_rn(y * qscale) (no beta)
+template <bool E4M3>
 __global__ void __launch_bounds__(256) rmsnorm_silu_cl_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx,
                                                               const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                              __nv_bfloat16* __restrict__ out, int64_t ldo, int64_t npix,
-                                                              int C, int apply_silu) {
+                                                              void* __restrict__ out, int64_t ldo, int64_t npix,
+                                                              int C, int apply_silu, float qscale) {
   const int64_t pix = int64_t(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (pix >= npix) return;
   const int lane = threadIdx.x & 31;
@@ -33,7 +38,8 @@ __global__ void __launch_bounds__(256) rmsnorm_silu_cl_kernel(const __nv_bfloat1
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
   const float denom = fmaxf(sqrtf(ss), 1e-12f);
   const float scale = sqrtf(float(C));
-  __nv_bfloat16* orow = out + pix * ldo;
+  __nv_bfloat16* orow = static_cast<__nv_bfloat16*>(out) + pix * ldo;
+  uint8_t* qrow = static_cast<uint8_t*>(out) + pix * ldo;
   for (int ch = lane; ch < nch; ch += 32) {
     const uint4 u = reinterpret_cast<const uint4*>(xr)[ch];
     const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
@@ -47,16 +53,29 @@ __global__ void __launch_bounds__(256) rmsnorm_silu_cl_kernel(const __nv_bfloat1
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       float v = __fmul_rn(__fmul_rn(__fdiv_rn(y[i], denom), scale), __ldg(gamma + ch * 8 + i));
-      if (beta) v = __fadd_rn(v, __ldg(beta + ch * 8 + i));
+      if (!E4M3 && beta) v = __fadd_rn(v, __ldg(beta + ch * 8 + i));
       if (apply_silu) v = __fdividef(v, 1.0f + __expf(-v));
       y[i] = v;
     }
-    uint4 o;
-    o.x = pack_bf16x2(y[0], y[1]);
-    o.y = pack_bf16x2(y[2], y[3]);
-    o.z = pack_bf16x2(y[4], y[5]);
-    o.w = pack_bf16x2(y[6], y[7]);
-    reinterpret_cast<uint4*>(orow)[ch] = o;
+    if constexpr (E4M3) {
+      uint32_t w[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(y[4 * i], qscale), __fmul_rn(y[4 * i + 1], qscale)),
+                                                     __NV_SATFINITE, __NV_E4M3);
+        const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(__fmul_rn(y[4 * i + 2], qscale), __fmul_rn(y[4 * i + 3], qscale)),
+                                                     __NV_SATFINITE, __NV_E4M3);
+        w[i] = lo | (hi << 16);
+      }
+      reinterpret_cast<uint2*>(qrow)[ch] = make_uint2(w[0], w[1]);
+    } else {
+      uint4 o;
+      o.x = pack_bf16x2(y[0], y[1]);
+      o.y = pack_bf16x2(y[2], y[3]);
+      o.z = pack_bf16x2(y[4], y[5]);
+      o.w = pack_bf16x2(y[6], y[7]);
+      reinterpret_cast<uint4*>(orow)[ch] = o;
+    }
   }
 }
 
@@ -135,9 +154,21 @@ using namespace fvb;
 extern "C" int fvb_rmsnorm_silu_cl(const void* x, int64_t ldx, const float* gamma, const float* beta, void* out,
                                    int64_t ldo, int64_t npix, int C, int apply_silu, void* stream) {
   FVB_CHECK_ARG(x && gamma && out && npix > 0 && C > 0 && C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0, "bad arguments");
-  rmsnorm_silu_cl_kernel<<<(unsigned)((npix + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), ldx, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out), ldo, npix, C,
-      apply_silu);
+  rmsnorm_silu_cl_kernel<false><<<(unsigned)((npix + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), ldx, gamma, beta, out, ldo, npix, C, apply_silu, 0.f);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+extern "C" int fvb_rmsnorm_silu_cl_e4m3(const void* x, int64_t ldx, const float* gamma, void* out, int64_t ldo, int64_t npix,
+                                        int C, int apply_silu, float bound, void* stream) {
+  FVB_CHECK_ARG(x && gamma && out && npix > 0 && C > 0 && C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0, "bad arguments");
+  FVB_CHECK_ARG(bound >= 0.f, "bound must be >= 0");
+  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+                "x must be 16-byte and out 8-byte aligned");
+  const float qscale = bound > 0.f ? 448.0f / bound : 0.f;
+  rmsnorm_silu_cl_kernel<true><<<(unsigned)((npix + 7) / 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), ldx, gamma, nullptr, out, ldo, npix, C, apply_silu, qscale);
   FVB_CHECK_CUDA(cudaGetLastError());
   return FVB_OK;
 }

@@ -728,6 +728,122 @@ def rmsnorm_silu_cl(x: torch.Tensor, gamma: torch.Tensor, beta=None, silu: bool 
     return out
 
 
+# ---------------------------------------------------------------- FP8 (e4m3) residual-block convolutions
+def rms_norm_e4m3_bound(gamma: torch.Tensor) -> float:
+    """Static e4m3 scale bound of a WanRMS_norm (+ SiLU) output: |v_c| <= sqrt(C) * max|gamma| (fp32)."""
+    C = gamma.numel()
+    return float(torch.tensor(C, dtype=torch.float32).sqrt() * gamma.detach().float().abs().max().cpu())
+
+
+def e4m3_x_scale(bound: float) -> float:
+    """The dequantisation scale a convolution applies to an input quantised against `bound`: bound / 448 (fp32), 1 if 0."""
+    if bound == 0.0:
+        return 1.0
+    return float(torch.tensor(bound, dtype=torch.float32) / torch.tensor(FP8_E4M3_MAX, dtype=torch.float32))
+
+
+def pack_conv_weight_fp8(w: torch.Tensor):
+    """pack_conv_weight, then one e4m3 scale per output channel (fvb_quantize_fp8_rows of the packed bf16 rows; the zero
+    padding does not change the amax) -> (q float8_e4m3fn [Cout, ntaps * Cin_pad], scale fp32 [Cout], Cin_pad, k)."""
+    packed, cin_pad, k = pack_conv_weight(w)
+    q, scale = quantize_fp8_rows(packed)
+    return q.contiguous(), scale, cin_pad, k
+
+
+def _require_e4m3(t: torch.Tensor, name: str) -> None:
+    if not t.is_cuda:
+        raise FvbError(f"{name} must be a CUDA tensor (no CPU fallback)")
+    if t.dtype != torch.float8_e4m3fn:
+        raise FvbError(f"{name} must be float8_e4m3fn, got {t.dtype}")
+
+
+def _norm_out(norm_out, shape, norm_bound, device):
+    dt = torch.bfloat16 if norm_bound is None else torch.float8_e4m3fn
+    if norm_out is None:
+        norm_out = torch.empty(shape, dtype=dt, device=device)
+    assert norm_out.shape == shape and norm_out.is_contiguous() and norm_out.dtype == dt
+    return norm_out
+
+
+def conv3d_cl_fp8(x: torch.Tensor, wq: torch.Tensor, w_scale: torch.Tensor, cin_pad: int, k: tuple, x_scale: float,
+                  bias=None, resid=None, out=None, T_out: int | None = None, t_off: int = 0) -> torch.Tensor:
+    """conv3d_cl on e4m3 operands (fvb_conv3d_cl_fp8): x float8_e4m3fn [T_in, H, W, Cin] read as x * x_scale, wq / w_scale
+    from pack_conv_weight_fp8. Output bf16 [T_out, H, W, Cout]."""
+    _require_e4m3(x, "x")
+    _require_e4m3(wq, "wq")
+    assert x.is_contiguous() and x.dim() == 4
+    T_in, H, W, Cin = x.shape
+    Cout = wq.shape[0]
+    kt, kh, kw = k
+    if T_out is None:
+        T_out = T_in - t_off
+    if out is None:
+        out = torch.empty((T_out, H, W, Cout), dtype=torch.bfloat16, device=x.device)
+    check(lib().fvb_conv3d_cl_fp8(ptr(x), c_int(T_in), c_int(H), c_int(W), c_int(Cin), c_float(x_scale), ptr(wq), _f32p(w_scale),
+                                  c_int(cin_pad), c_int(Cout), c_int(kt), c_int(kh), c_int(kw), ptr(bias), ptr(resid),
+                                  c_int64(resid.shape[-1] if resid is not None else 0), ptr(out), c_int64(out.shape[-1]),
+                                  c_int(T_out), c_int(t_off), stream_ptr()))
+    return out
+
+
+def conv3d_cl_fp8_norm(x: torch.Tensor, wq: torch.Tensor, w_scale: torch.Tensor, cin_pad: int, k: tuple, x_scale: float,
+                       gamma: torch.Tensor, bias=None, resid=None, want_raw: bool = True, silu: bool = True,
+                       T_out: int | None = None, t_off: int = 0, norm_out=None, norm_bound: float | None = None):
+    """conv3d_cl_fp8 with the consumer's RMS-norm (+ SiLU) fused (fvb_conv3d_cl_fp8_norm). Returns (raw bf16 or None,
+    normed): normed is bf16, or e4m3 quantised against norm_bound when one is given."""
+    _require_e4m3(x, "x")
+    _require_e4m3(wq, "wq")
+    assert x.is_contiguous() and x.dim() == 4
+    T_in, H, W, Cin = x.shape
+    Cout = wq.shape[0]
+    kt, kh, kw = k
+    if T_out is None:
+        T_out = T_in - t_off
+    assert gamma.dtype == torch.float32 and gamma.numel() == Cout and gamma.is_cuda
+    raw = torch.empty((T_out, H, W, Cout), dtype=torch.bfloat16, device=x.device) if want_raw else None
+    norm_out = _norm_out(norm_out, (T_out, H, W, Cout), norm_bound, x.device)
+    check(lib().fvb_conv3d_cl_fp8_norm(ptr(x), c_int(T_in), c_int(H), c_int(W), c_int(Cin), c_float(x_scale), ptr(wq),
+                                       _f32p(w_scale), c_int(cin_pad), c_int(Cout), c_int(kt), c_int(kh), c_int(kw), ptr(bias),
+                                       ptr(resid), c_int64(resid.shape[-1] if resid is not None else 0), ptr(raw), c_int64(Cout),
+                                       c_int(T_out), c_int(t_off), _f32p(gamma), ptr(norm_out), c_int64(Cout), c_int(int(silu)),
+                                       c_int(int(norm_bound is not None)), c_float(norm_bound or 0.0), stream_ptr()))
+    return raw, norm_out
+
+
+def conv3d_cl_norm_e4m3(x: torch.Tensor, w_packed: torch.Tensor, cin_pad: int, k: tuple, gamma: torch.Tensor,
+                        norm_bound: float, bias=None, resid=None, want_raw: bool = True, silu: bool = True,
+                        T_out: int | None = None, t_off: int = 0, norm_out=None):
+    """conv3d_cl_norm (bf16 operands) writing the normalised output as e4m3 against norm_bound (fvb_conv3d_cl_norm_e4m3)."""
+    _require_cuda_bf16(x, "x")
+    assert x.is_contiguous() and x.dim() == 4
+    T_in, H, W, Cin = x.shape
+    Cout = w_packed.shape[0]
+    kt, kh, kw = k
+    if T_out is None:
+        T_out = T_in - t_off
+    assert gamma.dtype == torch.float32 and gamma.numel() == Cout and gamma.is_cuda
+    raw = torch.empty((T_out, H, W, Cout), dtype=torch.bfloat16, device=x.device) if want_raw else None
+    norm_out = _norm_out(norm_out, (T_out, H, W, Cout), norm_bound, x.device)
+    check(lib().fvb_conv3d_cl_norm_e4m3(ptr(x), c_int(T_in), c_int(H), c_int(W), c_int(Cin), ptr(w_packed), c_int(cin_pad),
+                                        c_int(Cout), c_int(kt), c_int(kh), c_int(kw), ptr(bias), ptr(resid),
+                                        c_int64(resid.shape[-1] if resid is not None else 0), ptr(raw), c_int64(Cout),
+                                        c_int(T_out), c_int(t_off), _f32p(gamma), ptr(norm_out), c_int64(Cout), c_int(int(silu)),
+                                        c_float(norm_bound), stream_ptr()))
+    return raw, norm_out
+
+
+def rmsnorm_silu_cl_e4m3(x: torch.Tensor, gamma: torch.Tensor, bound: float, silu: bool = True, out=None) -> torch.Tensor:
+    """rmsnorm_silu_cl (no beta) written as e4m3: q = satfinite(v * 448 / bound) (fvb_rmsnorm_silu_cl_e4m3)."""
+    _require_cuda_bf16(x, "x")
+    C = x.shape[-1]
+    assert x.is_contiguous() and gamma.dtype == torch.float32 and gamma.numel() == C
+    out = _norm_out(out, tuple(x.shape), bound, x.device)
+    npix = x.numel() // C
+    check(lib().fvb_rmsnorm_silu_cl_e4m3(ptr(x), c_int64(C), _f32p(gamma), ptr(out), c_int64(C), c_int64(npix), c_int(C),
+                                         c_int(int(silu)), c_float(bound), stream_ptr()))
+    return out
+
+
 def upsample2x_cl(x: torch.Tensor) -> torch.Tensor:
     T, H, W, C = x.shape
     out = torch.empty((T, 2 * H, 2 * W, C), dtype=torch.bfloat16, device=x.device)

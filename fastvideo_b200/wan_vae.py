@@ -32,6 +32,9 @@ class WanVAEConfig:
     num_res_blocks: int = 2
     temperal_downsample: tuple = (False, True, True)
     out_channels: int = 3
+    # Decoder only: conv1 / conv2 of every residual block on e4m3 operands (fvb_conv3d_cl_fp8) with a static activation
+    # scale from the producing norm's gamma. Changes the output visibly; bf16 is the default.
+    fp8_convs: bool = False
 
 
 # fused consumer-norm epilogue (fvb_conv3d_cl_norm); FVB_VAE_FUSE_NORM=0/1 overrides (A/B measurements)
@@ -44,12 +47,23 @@ class _Conv:
     The feature cache of a causal convolution (its last two INPUT frames, wanvae.py:160-207) is the head of a persistent
     input buffer [2 + Tn, H, W, Cin]: producers write the new frames straight behind the cached ones (`in_view`), the kernel
     reads the contiguous slice [cached | new], and afterwards the last two frames move to the head -- instead of a
-    torch.cat of cache and input plus a clone per call (5 % of the decode in round 1)."""
+    torch.cat of cache and input plus a clone per call (5 % of the decode in round 1).
+
+    fp8_bound (FP8 residual-block convolution): the static bound of the norm that produces this convolution's input. The
+    weights are then e4m3 with one scale per output channel (no bf16 copy kept), the input buffer and cache are e4m3, every
+    producer writes e4m3 against that bound (`in_bound`), and the kernel reads it back with x_scale = bound / 448."""
     dtype = torch.bfloat16
 
-    def __init__(self, sd, name):
+    def __init__(self, sd, name, fp8_bound=None):
         w = sd[name + ".weight"]
-        self.w, self.cin_pad, self.k = ops.pack_conv_weight(w)
+        self.fp8 = fp8_bound is not None
+        self.in_bound = fp8_bound
+        if self.fp8:
+            self.w, self.w_scale, self.cin_pad, self.k = ops.pack_conv_weight_fp8(w)
+            self.x_scale = ops.e4m3_x_scale(fp8_bound)
+            self.dtype = torch.float8_e4m3fn
+        else:
+            self.w, self.cin_pad, self.k = ops.pack_conv_weight(w)
         self.bias = sd[name + ".bias"].to(torch.bfloat16).contiguous()
         self.cin, self.cout = w.shape[1], w.shape[0]
         self.buf = None   # [2 + Tn, H, W, Cin]; frames [2 - n_c, 2) are the cache
@@ -78,12 +92,15 @@ class _Conv:
         return b[2:2 + Tn]
 
     def __call__(self, x, resid=None, use_cache=True, interleave=False, norm=None, want_raw=True):
-        """x: [Tn, H, W, Cin] new frames. Causal in time when kt == 3. norm = (gamma, silu[, dest_fn]) asks for the CONSUMER's
-        RMS-norm (+ SiLU) of the output as well: the result is then (raw or None, normed) -- fused into the convolution's
-        epilogue when one tile holds a whole channel row (Cout <= 192), else a separate row pass; dest_fn(T, H, W, device)
-        may name the buffer the normalised frames go to (the consumer's in_view)."""
+        """x: [Tn, H, W, Cin] new frames. Causal in time when kt == 3. norm = (gamma, silu[, dest_fn[, bound]]) asks for the
+        CONSUMER's RMS-norm (+ SiLU) of the output as well: the result is then (raw or None, normed) -- fused into the
+        convolution's epilogue when one tile holds a whole channel row (Cout <= 192), else a separate row pass;
+        dest_fn(T, H, W, device) may name the buffer the normalised frames go to (the consumer's in_view); a bound that is not
+        None makes the normalised frames e4m3 (the consumer is an FP8 convolution)."""
         kt = self.k[0]
         Tn, H, W, _ = x.shape
+        if (x.dtype == torch.float8_e4m3fn) != self.fp8:
+            raise ops.FvbError(f"{'e4m3' if self.fp8 else 'bf16'} convolution given {x.dtype} input")
         if kt == 1 or not use_cache or self.stateless:
             # stateless: the frames before this call's first one are zeros (TMA out-of-bounds fill) = F.pad(x, 2 * pt)
             buf, n_c = x, 0
@@ -95,20 +112,40 @@ class _Conv:
             buf = self.buf[2 - n_c:2 + Tn]
         fuse = norm is not None and not interleave and 16 < self.cout <= ops.CONV_NORM_MAX_COUT and FUSE_NORM
         dest = norm[2](Tn, H, W, x.device) if norm is not None and len(norm) > 2 and norm[2] is not None else None
-        if fuse:
+        qb = norm[3] if norm is not None and len(norm) > 3 else None
+        if fuse and self.fp8:
+            out = ops.conv3d_cl_fp8_norm(buf, self.w, self.w_scale, self.cin_pad, self.k, self.x_scale, norm[0], self.bias, resid,
+                                         want_raw=want_raw, silu=norm[1], T_out=Tn, t_off=n_c, norm_out=dest, norm_bound=qb)
+        elif fuse and qb is not None:
+            out = ops.conv3d_cl_norm_e4m3(buf, self.w, self.cin_pad, self.k, norm[0], qb, self.bias, resid, want_raw=want_raw,
+                                          silu=norm[1], T_out=Tn, t_off=n_c, norm_out=dest)
+        elif fuse:
             out = ops.conv3d_cl_norm(buf, self.w, self.cin_pad, self.k, norm[0], self.bias, resid, want_raw=want_raw,
                                      silu=norm[1], T_out=Tn, t_off=n_c, norm_out=dest)
         else:
-            out = ops.conv3d_cl(buf, self.w, self.cin_pad, self.k, self.bias, resid, T_out=Tn, t_off=n_c,
-                                interleave_c=self.cout // 2 if interleave else 0)
+            if self.fp8:
+                out = ops.conv3d_cl_fp8(buf, self.w, self.w_scale, self.cin_pad, self.k, self.x_scale, self.bias, resid,
+                                        T_out=Tn, t_off=n_c)
+            else:
+                out = ops.conv3d_cl(buf, self.w, self.cin_pad, self.k, self.bias, resid, T_out=Tn, t_off=n_c,
+                                    interleave_c=self.cout // 2 if interleave else 0)
             if norm is not None:
-                out = (out, ops.rmsnorm_silu_cl(out, norm[0], silu=norm[1], out=dest))
+                out = (out, _norm(out, norm, out=dest))
         if kt == 3 and use_cache and not self.stateless:  # the stream's last two frames become the head of the buffer
             keep = min(2, n_c + Tn)
             src = self.buf[2 + Tn - keep:2 + Tn]
             self.buf[2 - keep:2] = src.clone() if Tn < 2 else src  # Tn == 1: source and destination overlap
             self.n_c = keep
         return out
+
+
+def _norm(x, norm, out=None):
+    """The consumer's RMS-norm (+ SiLU) as a separate row pass: norm = (gamma, silu[, dest_fn[, bound]]); e4m3 against
+    the bound when there is one."""
+    bound = norm[3] if len(norm) > 3 else None
+    if bound is not None:
+        return ops.rmsnorm_silu_cl_e4m3(x, norm[0], bound, silu=norm[1], out=out)
+    return ops.rmsnorm_silu_cl(x, norm[0], silu=norm[1], out=out)
 
 
 class _Linear1x1:
@@ -127,17 +164,18 @@ class _Linear1x1:
 
 
 class _ResBlock:
-    def __init__(self, sd, p, in_dim, out_dim):
+    def __init__(self, sd, p, in_dim, out_dim, fp8=False):
         self.g1 = sd[p + "norm1.gamma"].float().reshape(-1).contiguous()
         self.g2 = sd[p + "norm2.gamma"].float().reshape(-1).contiguous()
-        self.conv1, self.conv2 = _Conv(sd, p + "conv1"), _Conv(sd, p + "conv2")
+        b1, b2 = (ops.rms_norm_e4m3_bound(self.g1), ops.rms_norm_e4m3_bound(self.g2)) if fp8 else (None, None)
+        self.conv1, self.conv2 = _Conv(sd, p + "conv1", b1), _Conv(sd, p + "conv2", b2)
         self.shortcut = _Linear1x1(sd, p + "conv_shortcut") if in_dim != out_dim else None
 
     def convs(self):
         return [self.conv1, self.conv2]
 
     def first_norm(self):
-        return (self.g1, True, self.conv1.in_view)
+        return (self.g1, True, self.conv1.in_view, self.conv1.in_bound)
 
     def __call__(self, x, xn=None, next_norm=None):
         """xn: norm1+SiLU of x if the producer already made it; next_norm: (gamma, silu[, dest_fn]) of the consumer of this
@@ -145,9 +183,9 @@ class _ResBlock:
         Tn, H, W, _ = x.shape
         h = self.shortcut(x) if self.shortcut is not None else x
         if xn is None:
-            xn = ops.rmsnorm_silu_cl(x, self.g1, out=self.conv1.in_view(Tn, H, W, x.device))
+            xn = _norm(x, self.first_norm(), out=self.conv1.in_view(Tn, H, W, x.device))
         # conv1's output is only ever read through norm2 + SiLU, and only by conv2: written straight into conv2's input buffer
-        _, yn = self.conv1(xn, norm=(self.g2, True, self.conv2.in_view), want_raw=False)
+        _, yn = self.conv1(xn, norm=(self.g2, True, self.conv2.in_view, self.conv2.in_bound), want_raw=False)
         if next_norm is None:
             return self.conv2(yn, resid=h), None
         return self.conv2(yn, resid=h, norm=next_norm)
@@ -175,7 +213,7 @@ class _Attention:
             y = ops.linear(o, self.proj.w, self.proj.b, ops.EPI_RESID_BF16, resid=xt)
             outs.append(y.view(1, H, W, C))
         y = torch.cat(outs, 0) if T > 1 else outs[0]
-        return y, (ops.rmsnorm_silu_cl(y, next_norm[0], silu=next_norm[1]) if next_norm is not None else None)
+        return y, (_norm(y, next_norm) if next_norm is not None else None)
 
 
 def _run_chain(mods, x, final_norm=None, xn=None):
@@ -265,6 +303,8 @@ class WanVAEEncoder:
     1x1 convolutions and the mid-block attention); parameter names are the reference's."""
 
     def __init__(self, cfg: WanVAEConfig, state_dict: dict):
+        if cfg.fp8_convs:
+            raise ops.FvbError("WanVAEConfig.fp8_convs applies to the decoder only; the encoder has no FP8 path")
         sd = dict(state_dict)
         self.cfg = cfg
         dim, mult = cfg.base_dim, list(cfg.dim_mult)
@@ -337,8 +377,9 @@ class WanVAEDecoder:
         self.post_quant = _Linear1x1(sd, "post_quant_conv")
         d = "decoder."
         self.conv_in = _Conv(sd, d + "conv_in")
-        self.mid = [_ResBlock(sd, d + "mid_block.resnets.0.", dims[0], dims[0]), _Attention(sd, d + "mid_block.attentions.0."),
-                    _ResBlock(sd, d + "mid_block.resnets.1.", dims[0], dims[0])]
+        fp8 = cfg.fp8_convs
+        self.mid = [_ResBlock(sd, d + "mid_block.resnets.0.", dims[0], dims[0], fp8), _Attention(sd, d + "mid_block.attentions.0."),
+                    _ResBlock(sd, d + "mid_block.resnets.1.", dims[0], dims[0], fp8)]
         self.ups = []
         for i, (in_dim, out_dim) in enumerate(zip(dims[:-1], dims[1:])):
             if i > 0:
@@ -346,7 +387,7 @@ class WanVAEDecoder:
             blocks = []
             cur = in_dim
             for j in range(cfg.num_res_blocks + 1):
-                blocks.append(_ResBlock(sd, f"{d}up_blocks.{i}.resnets.{j}.", cur, out_dim))
+                blocks.append(_ResBlock(sd, f"{d}up_blocks.{i}.resnets.{j}.", cur, out_dim, fp8))
                 cur = out_dim
             if i != len(mult) - 1:
                 mode = "upsample3d" if temperal_upsample[i] else "upsample2d"

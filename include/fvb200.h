@@ -393,6 +393,47 @@ int fvb_conv3d_cl_norm(const void* x, int T_in, int H, int W, int Cin, const voi
 int fvb_rmsnorm_silu_cl(const void* x, int64_t ldx, const float* gamma, const float* beta, void* out, int64_t ldo,
                         int64_t npix, int C, int apply_silu, void* stream);
 
+/* --------------------------------------------------------------------------------------------
+ * FP8 (e4m3) residual-block convolutions of the Wan VAE decoder
+ *
+ * Static activation scale. Every conv1 / conv2 of a WanResidualBlock reads v = silu?(y / ||y|| * sqrt(C) * gamma), so
+ * |v_c| <= bound = sqrt(C) * max_c |gamma_c| (SiLU never raises the magnitude). The norm that produces v writes it as
+ *   q = e4m3_satfinite_rn(v * inv),  inv = 448.0f / bound (IEEE fp32 division);  bound == 0: inv = 0 (q = 0)
+ * and the convolution reads it with x_scale = bound / 448 (1 when bound == 0). satfinite absorbs the last-ulp overshoot of
+ * the rounded norm. No amax pass; the scale is known when the weights are loaded.
+ *
+ * fvb_conv3d_cl_fp8: fvb_conv3d_cl with x e4m3 [T_in][H][W][Cin] (Cin % 16 == 0: 16-byte pixel rows) and
+ *   w_packed e4m3 [Cout][kt*kh*kw][Cin_pad] with w_scale fp32 [Cout] (fvb_quantize_fp8_rows of the packed bf16 weight:
+ *   one scale per output channel; the zero padding does not change the amax):
+ *   acc = sum over taps and channels of x * w            (wgmma .e4m3 products, fp32 accumulators in the tensor core)
+ *   y = bf16(((acc * x_scale) * w_scale[n]) + bias[n]);  out = bf16(y + resid) if resid  (as fvb_conv3d_cl)
+ *   No interleave_c.
+ * fvb_conv3d_cl_fp8_norm: the same with the consumer's norm fused as in fvb_conv3d_cl_norm (16 < Cout <= 192);
+ *   norm_e4m3 == 0: norm_out bf16; norm_e4m3 != 0: norm_out e4m3 = e4m3_satfinite_rn(normed * (448 / norm_bound)),
+ *   normed the fp32 value the bf16 output would round (norm_ld % 16 == 0).
+ * fvb_conv3d_cl_norm_e4m3: fvb_conv3d_cl_norm (bf16 operands) writing its normalised output as e4m3 by the same rule
+ *   (the upsampler convolution that feeds a residual block).
+ * fvb_rmsnorm_silu_cl_e4m3: fvb_rmsnorm_silu_cl (no beta) writing e4m3 by the same rule; the separate pass for
+ *   Cout > 192 and after the mid-block attention.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_conv3d_cl_fp8(const void* x, int T_in, int H, int W, int Cin, float x_scale, const void* w_packed,
+                      const float* w_scale, int Cin_pad, int Cout, int kt, int kh, int kw, const void* bias,
+                      const void* resid, int64_t resid_ld, void* out, int64_t out_ld, int T_out, int t_off, void* stream);
+
+int fvb_conv3d_cl_fp8_norm(const void* x, int T_in, int H, int W, int Cin, float x_scale, const void* w_packed,
+                           const float* w_scale, int Cin_pad, int Cout, int kt, int kh, int kw, const void* bias,
+                           const void* resid, int64_t resid_ld, void* out, int64_t out_ld, int T_out, int t_off,
+                           const float* norm_gamma, void* norm_out, int64_t norm_ld, int norm_silu, int norm_e4m3,
+                           float norm_bound, void* stream);
+
+int fvb_conv3d_cl_norm_e4m3(const void* x, int T_in, int H, int W, int Cin, const void* w_packed, int Cin_pad, int Cout,
+                            int kt, int kh, int kw, const void* bias, const void* resid, int64_t resid_ld, void* out,
+                            int64_t out_ld, int T_out, int t_off, const float* norm_gamma, void* norm_out, int64_t norm_ld,
+                            int norm_silu, float norm_bound, void* stream);
+
+int fvb_rmsnorm_silu_cl_e4m3(const void* x, int64_t ldx, const float* gamma, void* out, int64_t ldo, int64_t npix, int C,
+                             int apply_silu, float bound, void* stream);
+
 /* nearest-exact 2x spatial upsample of [T][H][W][C] -> [T][2H][2W][C] (WanUpsample, wanvae.py:236-248). */
 int fvb_upsample2x_cl(const void* in, void* out, int T, int H, int W, int C, void* stream);
 
