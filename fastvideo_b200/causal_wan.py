@@ -242,27 +242,27 @@ def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb
     kw = _roped_window(cache, k0, k1, cos, sin, d) if rel else cache.k[k0:k1]
     a = ops.attention(q.view(1, S, H, d), kw.unsqueeze(0), cache.v[k0:k1].unsqueeze(0), softmax_scale=d ** -0.5)
     # to_out + per-frame gated residual (bf16 product), then LayerNorm(affine) of the bf16 residual (layernorm.py:159-213)
-    x = ops.linear(a.reshape(S, D), blk.w_o, blk.b_o, ops.EPI_RESID_GATE_BF16R, resid=x, gate=gate_msa, gate_rows=tpf)
+    x = ops.linear_any(a.reshape(S, D), blk.w_o, blk.b_o, ops.EPI_RESID_GATE_BF16R, resid=x, gate=gate_msa, gate_rows=tpf)
     n2 = ops.layernorm_modulate(x, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps)
 
     # 2. cross-attention, text K/V cached across the rollout (wanvideo.py:188-222)
-    q2 = ops.linear(n2, blk.w_q2, blk.b_q2)
+    q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
     ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
     if xcache is not None and xcache.kv is not None:
         kv2 = xcache.kv
     else:
-        kv2 = ops.linear(ctx, blk.w_kv2, blk.b_kv2)
+        kv2 = ops.linear_any(ctx, blk.w_kv2, blk.b_kv2)
         ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
         if xcache is not None:
             xcache.kv = kv2
     a2 = ops.attention(q2.unflatten(1, (H, d)).unsqueeze(0), kv2[:, :D].unflatten(1, (H, d)).unsqueeze(0),
                        kv2[:, D:].unflatten(1, (H, d)).unsqueeze(0), softmax_scale=d ** -0.5).reshape(S, D)
-    x = ops.linear(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
+    x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
     n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps, mod_rows=tpf, mod_bf16=True)
 
     # 3. feed-forward + per-frame gated residual (causal_wanvideo.py:338-340)
-    f = ops.linear(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-    return ops.linear(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=tpf)
+    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+    return ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=tpf)
 
 
 def _require_bf16_model(cfg: WanDiTConfig) -> None:
@@ -441,7 +441,7 @@ class SPCausalWanDiT:
         frame_row = []
         for p0, p1 in segs:
             frame_row += list(range(p0, p1, fs))
-        qk = ops.linear(n1, blk.w_qkv[:2 * D], blk.b_qkv[:2 * D])  # local [S_loc, 2D]: RMSNorm needs whole rows
+        qk = ops.linear_any(n1, blk.w_qkv[:2 * D], blk.b_qkv[:2 * D])  # local [S_loc, 2D]: RMSNorm needs whole rows
         slab, rowb = st["slab"], Hl * d
         q_base, k_base, v_base = st["q"].data_ptr(), cache.k.data_ptr(), cache.v.data_ptr()
         v_off = st["head_off"] + (v_base - slab.data_ptr()) // 2
@@ -470,21 +470,21 @@ class SPCausalWanDiT:
                       x_seg_stride=S_loc * rowb, resid=x, gate=gate_msa, gate_rows=n)
         x = y
         n2 = ops.layernorm_modulate(x, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps)
-        q2 = ops.linear(n2, blk.w_q2, blk.b_q2)
+        q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
         ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
         if xcache is not None and xcache.kv is not None:
             kv2 = xcache.kv
         else:
-            kv2 = ops.linear(ctx, blk.w_kv2, blk.b_kv2)
+            kv2 = ops.linear_any(ctx, blk.w_kv2, blk.b_kv2)
             ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
             if xcache is not None:
                 xcache.kv = kv2
         a2 = ops.attention(q2.unflatten(1, (H, d)).unsqueeze(0), kv2[:, :D].unflatten(1, (H, d)).unsqueeze(0),
                            kv2[:, D:].unflatten(1, (H, d)).unsqueeze(0), softmax_scale=d ** -0.5).reshape(S_loc, D)
-        x = ops.linear(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
+        x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
         n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps, mod_rows=n, mod_bf16=True)
-        f_ = ops.linear(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-        return ops.linear(f_, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=n)
+        f_ = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+        return ops.linear_any(f_, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=n)
 
     @torch.no_grad()
     def forward_inference(self, latents, text, timestep, kv_cache, crossattn_cache, current_start: int = 0, start_frame: int = 0):

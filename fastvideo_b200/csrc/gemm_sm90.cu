@@ -1,18 +1,22 @@
-// gemm_sm90.cu -- persistent, warp-specialised GEMM for sm_90a, bf16 or fp8 (e4m3) operands:
+// gemm_sm90.cu -- persistent, warp-specialised GEMM for sm_90a, bf16, fp8 (e4m3) or int8-weight operands:
 //   out = epilogue(x[M,K] @ w[N,K]^T + bias)                                   (bf16)
 //   out = epilogue((x_q[M,K] @ w_q[N,K]^T) * x_scale[m] * w_scale[n] + bias)   (e4m3, per-row / per-channel scales)
+//   out = epilogue((x[M,K] @ w_q[N,K]^T) * w_scale[n] + bias)                  (bf16 x, int8 w, per-channel scales)
 // TMA (128B swizzle) -> shared-memory ring -> wgmma (two warpgroups, 64 rows x BN each, fp32 accumulators in registers)
 // -> epilogue straight from the accumulator registers with fused bias / GELU(tanh) / gated residual.
 // A k-block is one 128-byte swizzle row of both operands: 64 bf16 or 128 e4m3 elements, so a stage holds the same bytes
 // for both types. The e4m3 tensor-core accumulator keeps fewer bits than fp32, so the fp8 path lets each k-block's MMAs
 // accumulate into a second register set and adds that into the fp32 accumulators once per k-block (every 128 elements).
+// The int8-weight path (W8) runs the bf16 MMAs: each k-block's BN x 64 int8 weight tile lands, unswizzled, in the second
+// half of the stage's bf16 B region, and warps 1-3 of the producer warpgroup widen it in place to the 128B-swizzled
+// bf16 tile the B descriptor reads. int8 -> bf16 is exact, so the products are those of a bf16 GEMM on integer weights.
 //
 // Stands behind fastvideo/layers/linear.py:146-156 (F.linear) and the elementwise op that follows
 // each linear in fastvideo/models/dits/wanvideo.py:394-431; rounding points mirror the reference's
 // eager bf16 path (see include/fvb200.h).
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1 and 2 = MMA + epilogue for rows
-// [0, 64) and [64, 128) of the 128-row tile. The producer runs ahead into the next tile while the consumers finish the
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues; on the W8 path warps 1-3 widen the weights),
+// warpgroups 1 and 2 = MMA + epilogue for rows [0, 64) and [64, 128) of the 128-row tile. The producer runs ahead into the next tile while the consumers finish the
 // epilogue of the current one.
 // Persistent CTAs walk the tiles in weight-stripe order (tile_coords): a stripe of 8 column tiles stays in L2 while
 // the row-blocks stream past it. Output column blocks may be redirected by an offset table (out_col_offsets), which
@@ -48,14 +52,15 @@ struct GemmParams {
   int stripe_n;  // > 0: weight-stripe raster with this many column tiles per stripe (see tile_coords)
 };
 
-// e4m3 operands: the per-row / per-channel scales. The bf16 kernels keep taking the plain GemmParams.
+// e4m3 / int8-weight operands: the per-row / per-channel scales (a_scale: e4m3 only). The bf16 kernels keep taking the
+// plain GemmParams.
 struct GemmParamsFp8 : GemmParams {
   const float* a_scale;  // [M]
   const float* b_scale;  // [N_valid]
   int N_valid;           // columns with a b_scale entry (N before rounding up to 8)
 };
-template <bool FP8>
-using GemmParamsT = std::conditional_t<FP8, GemmParamsFp8, GemmParams>;
+template <bool SCALED>
+using GemmParamsT = std::conditional_t<SCALED, GemmParamsFp8, GemmParams>;
 
 template <int BN>
 struct GemmCfg {
@@ -100,9 +105,67 @@ FVB_DEVICE float gelu_tanh_f(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
-template <int BN, int EPI, bool FP8>
+// W8: the int8 weight tile (BN rows of 64 bytes) sits in the upper half of the stage's bf16 B region
+template <int BN>
+constexpr int W8_STAGING_OFFSET = BN * GEMM_BK;
+constexpr int W8_CONVERT_THREADS = 96;  // warps 1-3 of the producer warpgroup
+
+FVB_DEVICE uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+FVB_DEVICE void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+
+// Widen one stage's int8 weight tile into the 128B-swizzled bf16 K-major tile the wgmma B descriptor reads, in place.
+// Unit u = 16 int8 weights (row u / 4, k [16 (u % 4), +16)) -> two 16-byte bf16 chunks of that row. Output row r covers
+// staging rows 2r - BN and 2r - BN + 1, which are <= r, so rows are processed in ascending batches: every thread loads its
+// units of the batch, the 96 threads meet at a named barrier, then they store; a batch never overwrites staging rows of
+// a later batch. sb: shared-space address of the stage's B region.
+template <int BN>
+FVB_DEVICE void w8_widen_tile(uint32_t sb, int t) {
+  constexpr int UNITS = BN * 4, PER = 2;  // units per thread per batch
+  const uint32_t stg = sb + W8_STAGING_OFFSET<BN>;
+#pragma unroll 1  // the producer warpgroup runs with 40 registers
+  for (int u0 = 0; u0 < UNITS; u0 += PER * W8_CONVERT_THREADS) {
+    uint4 v[PER];
+#pragma unroll
+    for (int p = 0; p < PER; ++p) {
+      const int u = u0 + p * W8_CONVERT_THREADS + t;
+      if (u < UNITS) v[p] = lds128(stg + u * 16);
+    }
+    named_bar_sync(1, W8_CONVERT_THREADS);
+#pragma unroll
+    for (int p = 0; p < PER; ++p) {
+      const int u = u0 + p * W8_CONVERT_THREADS + t;
+      if (u >= UNITS) continue;
+      const int r = u >> 2, q = u & 3;
+      const uint32_t w[4] = {v[p].x, v[p].y, v[p].z, v[p].w};
+      uint32_t o[8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        // int8 b -> fp32 exactly: the float with bits 0x4B0000uu (u = b ^ 0x80) is 2^23 + b + 128. |b| <= 128 has at
+        // most 8 significant bits, so its bf16 is the upper half of the fp32 bits (no rounding needed)
+        const uint32_t x = w[i] ^ 0x80808080u;
+        uint32_t f[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) f[j] = __float_as_uint(__uint_as_float(__byte_perm(x, 0x4B000000u, 0x7440 + j)) - 8388736.f);
+        o[2 * i] = __byte_perm(f[0], f[1], 0x7632);
+        o[2 * i + 1] = __byte_perm(f[2], f[3], 0x7632);
+      }
+      const uint32_t row = sb + r * 128;
+      sts128(row + (((2 * q) ^ (r & 7)) << 4), o[0], o[1], o[2], o[3]);
+      sts128(row + (((2 * q + 1) ^ (r & 7)) << 4), o[4], o[5], o[6], o[7]);
+    }
+  }
+}
+
+// FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); neither: bf16 x bf16
+template <int BN, int EPI, bool FP8, bool W8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8> p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8 || W8> p) {
   using Cfg = GemmCfg<BN>;
   constexpr int BK = FP8 ? GEMM_BK_FP8 : GEMM_BK;
   extern __shared__ uint8_t smem_raw[];
@@ -122,6 +185,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 8);  // lane 0 of each of the eight consumer warps
     }
+    if constexpr (W8)
+      for (int i = 0; i < Cfg::STAGES; ++i) mbar_init(&bars[2 * Cfg::STAGES + i], 1);  // `landed` below
     fence_mbar_init();
   }
   __syncthreads();
@@ -129,6 +194,41 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
     reg_dealloc<40>();
+    if constexpr (W8) {
+      // thread 0 issues the TMA loads onto `landed`; warps 1-3 widen each landed weight tile, then release the stage to
+      // the consumers on `full`
+      uint64_t* landed = bars + 2 * Cfg::STAGES;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        const int bt = tile / tiles_per_batch;
+        tile_coords(tile - bt * tiles_per_batch, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
+        for (int kb = 0; kb < p.num_k; ++kb) {
+          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+          uint8_t* sb = sa + Cfg::A_BYTES;
+          if (threadIdx.x == 0) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            mbar_expect_tx(&landed[stage], Cfg::A_BYTES + BN * GEMM_BK);
+            const int k0 = kb * GEMM_BK;
+            const int seg = k0 / p.a_seg_len;
+            tma_load_4d(sa, &tmA, &landed[stage], k0 - seg * p.a_seg_len, m_blk * GEMM_BM, seg, bt);
+            tma_load_3d(sb + W8_STAGING_OFFSET<BN>, &tmB, &landed[stage], k0, n_blk * BN, bt);
+          } else if (threadIdx.x >= 32) {
+            mbar_wait(&landed[stage], phase);
+            w8_widen_tile<BN>(smem_u32(sb), threadIdx.x - 32);
+            fence_proxy_async();  // the generic-proxy stores are read by wgmma (async proxy)
+            named_bar_sync(1, W8_CONVERT_THREADS);
+            if (threadIdx.x == 32) mbar_arrive(&full[stage]);
+          }
+          if (++stage == Cfg::STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+      return;
+    }
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -239,7 +339,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       float2 bf = make_float2(0.f, 0.f);
       if (p.bias != nullptr) bf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
       float2 sw = make_float2(1.f, 1.f);
-      if constexpr (FP8) {
+      if constexpr (FP8 || W8) {
         sw.x = col < p.N_valid ? __ldg(p.b_scale + col) : 0.f;
         sw.y = col + 1 < p.N_valid ? __ldg(p.b_scale + col + 1) : 0.f;
       }
@@ -251,6 +351,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if constexpr (FP8) {  // (acc * s_x[m]) * s_w[n], fp32 round-to-nearest, before the bias
           f0 = __fmul_rn(__fmul_rn(f0, sx[i]), sw.x);
           f1 = __fmul_rn(__fmul_rn(f1, sx[i]), sw.y);
+        } else if constexpr (W8) {  // acc * s_w[n], fp32 round-to-nearest, before the bias
+          f0 = __fmul_rn(f0, sw.x);
+          f1 = __fmul_rn(f1, sw.y);
         }
         if (p.bias != nullptr) {
           f0 = __fadd_rn(f0, bf.x);
@@ -296,10 +399,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
-template <int BN, int EPI, bool FP8>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8>& p, cudaStream_t st) {
+template <int BN, int EPI, bool FP8, bool W8 = false>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8 || W8>& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_kernel<BN, EPI, FP8>;
+  auto kern = gemm_kernel<BN, EPI, FP8, W8>;
   static bool configured = false;
   if (!configured) {
     FVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -327,18 +430,18 @@ static int dispatch_epi(int epi, const CUtensorMap& a, const CUtensorMap& b, con
   return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue%s");
 }
 
-// fp8 operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
-template <int BN>
-static int dispatch_epi_fp8(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsFp8& p, cudaStream_t st) {
+// fp8 / int8-weight operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
+template <int BN, bool FP8, bool W8>
+static int dispatch_epi_scaled(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsFp8& p, cudaStream_t st) {
   switch (epi) {
-    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, true>(a, b, p, st);
-    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, true>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, true>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, true>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, true>(a, b, p, st);
-    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, true>(a, b, p, st);
+    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, FP8, W8>(a, b, p, st);
+    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, FP8, W8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, FP8, W8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, FP8, W8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, FP8, W8>(a, b, p, st);
+    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, FP8, W8>(a, b, p, st);
   }
-  return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue for fvb_linear_fp8%s");
+  return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue for fvb_linear_fp8 / fvb_linear_w8_sp%s");
 }
 
 }  // namespace fvb
@@ -350,14 +453,20 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
                      const void* resid, int64_t ldr,
                      const float* gate, int gate_rows, int64_t gate_stride, float div, int M, int N, int K, int batch,
                      int epilogue, void* stream, const float* x_scale = nullptr, const float* w_scale = nullptr) {
-  // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales
+  // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales.
+  // w_scale alone: x is bf16 and w is int8 with per-output-channel fp32 scales.
   const bool fp8 = x_scale != nullptr;
+  const bool w8 = !fp8 && w_scale != nullptr;
   FVB_CHECK_ARG(x && w && out, "null pointer");
   FVB_CHECK_ARG(M > 0 && N > 0 && K > 0 && batch > 0, "empty problem");
   if (fp8) {
     FVB_CHECK_ARG(w_scale != nullptr, "w_scale required");
     FVB_CHECK_ARG(batch == 1 && a_seg_len <= 0 && out_col_offsets == nullptr, "fp8 operands: plain row-major, unbatched");
     FVB_CHECK_ARG(ldx % 16 == 0 && ldw % 16 == 0, "fp8 ldx/ldw must be multiples of 16 (16-byte rows)");
+  }
+  if (w8) {
+    FVB_CHECK_ARG(batch == 1, "int8 weights: unbatched");
+    FVB_CHECK_ARG(ldw % 16 == 0, "int8 ldw must be a multiple of 16 (16-byte rows)");
   }
   FVB_CHECK_ARG(ldx % 8 == 0 && ldw % 8 == 0 && ldo % 8 == 0, "ldx/ldw/ldo must be multiples of 8");
   // N not a multiple of 8: the tail columns up to the next multiple of 8 are written as zeros (they must fit in ldo)
@@ -382,6 +491,7 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
                      : (N >= 256 && N % 256 == 0) ? 256 : (N >= 128 && N % 128 == 0 ? 128 : (N >= 192 ? 256 : 64));
   const int BK = fp8 ? GEMM_BK_FP8 : GEMM_BK;
   const int esz = fp8 ? 1 : 2;  // operand element bytes
+  const int wsz = fp8 || w8 ? 1 : 2;
 
   CUtensorMap tmA, tmB;
   if (a_seg_len <= 0 || a_seg_len >= K) {
@@ -400,9 +510,12 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
   }
   {
     uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)batch};
-    uint64_t str[3] = {(uint64_t)esz, (uint64_t)ldw * esz, (uint64_t)(batch > 1 ? w_batch : ldw * (int64_t)N) * esz};
+    uint64_t str[3] = {(uint64_t)wsz, (uint64_t)ldw * wsz, (uint64_t)(batch > 1 ? w_batch : ldw * (int64_t)N) * wsz};
     uint32_t box[3] = {(uint32_t)BK, (uint32_t)BN, 1};
-    int r = fp8 ? make_tmap_u8(&tmB, w, 3, dims, str, box) : make_tmap_bf16(&tmB, w, 3, dims, str, box);
+    // int8 weights land unswizzled in a staging area and are widened into the swizzled bf16 layout in shared memory
+    int r = fp8  ? make_tmap_u8(&tmB, w, 3, dims, str, box)
+            : w8 ? make_tmap_u8(&tmB, w, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE)
+                 : make_tmap_bf16(&tmB, w, 3, dims, str, box);
     if (r) return r;
   }
   GemmParamsFp8 p;  // the bf16 kernels receive its GemmParams part
@@ -437,7 +550,14 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     p.stripe_n = 0;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (fp8) return BN == 128 ? dispatch_epi_fp8<128>(epilogue, tmA, tmB, p, st) : dispatch_epi_fp8<64>(epilogue, tmA, tmB, p, st);
+  if (fp8)
+    return BN == 128 ? dispatch_epi_scaled<128, true, false>(epilogue, tmA, tmB, p, st)
+                     : dispatch_epi_scaled<64, true, false>(epilogue, tmA, tmB, p, st);
+  if (w8) {
+    if (BN == 256) return dispatch_epi_scaled<256, false, true>(epilogue, tmA, tmB, p, st);
+    if (BN == 128) return dispatch_epi_scaled<128, false, true>(epilogue, tmA, tmB, p, st);
+    return dispatch_epi_scaled<64, false, true>(epilogue, tmA, tmB, p, st);
+  }
   if (BN == 256) return dispatch_epi<256>(epilogue, tmA, tmB, p, st);
   if (BN == 128) return dispatch_epi<128>(epilogue, tmA, tmB, p, st);
   return dispatch_epi<64>(epilogue, tmA, tmB, p, st);
@@ -481,4 +601,14 @@ extern "C" int fvb_linear_fp8(const void* xq, int64_t ldx, const float* x_scale,
   if (x_scale == nullptr || w_scale == nullptr) return set_error(FVB_ERR_INVALID_ARG, "invalid argument: x_scale and w_scale are required%s");
   return gemm_impl(xq, ldx, 0, 0, 0, wq, ldw, 0, bias, out, ldo, 0, nullptr, resid, ldr, gate, gate_rows, gate_stride, 1.0f,
                    M, N, K, 1, epilogue, stream, x_scale, w_scale);
+}
+
+extern "C" int fvb_linear_w8_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_stride, const void* wq, int64_t ldw,
+                                const float* w_scale, const void* bias, void* out, int64_t ldo, const int64_t* out_col_offsets,
+                                const void* resid, int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M,
+                                int N, int K, int epilogue, void* stream) {
+  if (w_scale == nullptr) return set_error(FVB_ERR_INVALID_ARG, "invalid argument: w_scale is required%s");
+  if (out_col_offsets != nullptr && N % 128 != 0) return set_error(FVB_ERR_INVALID_ARG, "column-block offsets need N %% 128 == 0%s");
+  return gemm_impl(x, ldx, 0, x_seg_len, x_seg_stride, wq, ldw, 0, bias, out, ldo, 0, out_col_offsets, resid, ldr, gate,
+                   gate_rows, gate_stride, 1.0f, M, N, K, 1, epilogue, stream, nullptr, w_scale);
 }

@@ -276,7 +276,7 @@ class SPWanDiT:
         # buffer of the rank that owns it (column-block offsets reaching into peer memory), so that half of the exchange
         # rides on the GEMM tile by tile. q and k go to a local buffer first (RMSNorm is over the full row).
         ops.linear_sp(n1, S_loc, D, n1.stride(0), blk.w_qkv[2 * D:], blk.b_qkv[2 * D:], recv, rs, out_col_offsets=st["vg_off"])
-        qk = ops.linear(n1, blk.w_qkv[:2 * D], blk.b_qkv[:2 * D])  # local [S_loc, 2D]
+        qk = ops.linear_any(n1, blk.w_qkv[:2 * D], blk.b_qkv[:2 * D])  # local [S_loc, 2D]
         base = recv.data_ptr()
         # q, k: RMSNorm + RoPE, every head written to its owner's receive buffer (projection p sits p*Hl*d further)
         ops.rmsnorm_rope_scatter(qk[:, :D], blk.norm_q, qk[:, D:], blk.norm_k, base, base + Hl * d * 2, rs, st["off"],
@@ -307,10 +307,10 @@ class SPWanDiT:
 
         from .wan_dit import cross_attention
         a2 = cross_attention(n2, blk, ctx, cfg)
-        x = ops.linear(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
+        x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
         n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps)
-        f = ops.linear(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-        return ops.linear(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
+        f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+        return ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
 
     @torch.no_grad()
     def forward(self, latents, text, timestep, vsa_sparsity=None):

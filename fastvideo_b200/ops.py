@@ -145,9 +145,93 @@ def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: torch.Tensor | None = None, 
     return out.reshape(*x.shape[:-1], N)
 
 
-def linear_any(x: torch.Tensor, w, *args, **kwargs) -> torch.Tensor:
-    """`linear_fp8` for an Fp8Weight, `linear` for a bf16 tensor."""
-    return (linear_fp8 if isinstance(w, Fp8Weight) else linear)(x, w, *args, **kwargs)
+class Int8Weight:
+    """A linear weight w[N, K] held as int8 rows with one fp32 scale per output channel (w ~= q * scale[:, None]); the
+    activations it multiplies stay bf16 (fvb_linear_w8_sp)."""
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor):
+        if q.dtype != torch.int8 or q.dim() != 2 or q.stride(1) != 1 or q.stride(0) % 16 != 0:
+            raise FvbError("Int8Weight.q must be int8 [N, K] with 16-byte-aligned rows")
+        if scale.dtype != torch.float32 or scale.shape != (q.shape[0],) or not scale.is_contiguous():
+            raise FvbError("Int8Weight.scale must be fp32 [N] contiguous")
+        if q.device != scale.device:
+            raise FvbError("Int8Weight.q and scale must be on the same device")
+        self.q, self.scale = q, scale
+
+    @classmethod
+    def quantize(cls, w: torch.Tensor) -> "Int8Weight":
+        """[N, K] -> per-output-channel int8, once at load (torch, on w's device): amax = max|w[n]| (fp32),
+        scale = amax / 127, q = clamp(rint(w * (127 / amax)), -127, 127); an all-zero row gets scale 1 and q = 0."""
+        if w.dim() != 2:
+            raise FvbError("Int8Weight.quantize takes a 2-D [N, K] weight")
+        N, K = w.shape
+        w32 = w.detach().float()
+        amax = w32.abs().amax(dim=1)
+        zero = amax == 0
+        one = torch.ones_like(amax)
+        inv = torch.where(zero, one, torch.full_like(amax, 127.0) / torch.where(zero, one, amax))
+        scale = torch.where(zero, one, amax / 127.0)
+        ld = (K + 15) // 16 * 16
+        q = torch.zeros((N, ld), dtype=torch.int8, device=w.device)
+        q[:, :K] = torch.clamp(torch.round(w32 * inv[:, None]), -127, 127).to(torch.int8)
+        return cls(q[:, :K], scale.contiguous())
+
+    def __getitem__(self, rows) -> "Int8Weight":
+        """Row slice w[a:b] (q rows and scale rows), e.g. the Q / K / V parts of a fused QKV weight."""
+        if not isinstance(rows, slice) or rows.step not in (None, 1):
+            raise FvbError("Int8Weight supports contiguous row slices only")
+        return Int8Weight(self.q[rows], self.scale[rows])
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    @property
+    def device(self):
+        return self.q.device
+
+    @property
+    def nbytes(self) -> int:
+        return self.q.numel() * self.q.element_size() + self.scale.numel() * 4
+
+    def dequantize(self) -> torch.Tensor:
+        """fp32 [N, K] values the GEMM multiplies with (q * scale)."""
+        return self.q.float() * self.scale[:, None]
+
+
+def linear_any(x: torch.Tensor, w, bias: torch.Tensor | None = None, epilogue: int = EPI_BIAS,
+               resid: torch.Tensor | None = None, gate: torch.Tensor | None = None,
+               out: torch.Tensor | None = None, gate_rows: int = 0) -> torch.Tensor:
+    """`linear` for whatever the weight holds: linear_fp8 for an Fp8Weight, fvb_linear_w8_sp for an Int8Weight,
+    `linear` for a bf16 tensor."""
+    if isinstance(w, Fp8Weight):
+        return linear_fp8(x, w, bias, epilogue, resid, gate, out, gate_rows)
+    if not isinstance(w, Int8Weight):
+        return linear(x, w, bias, epilogue, resid, gate, out, gate_rows)
+    _require_cuda_bf16(x, "x")
+    K = x.shape[-1]
+    N = w.shape[0]
+    if w.shape[1] != K:
+        raise FvbError(f"x has K={K}, weight has K={w.shape[1]}")
+    x2 = x.reshape(-1, K)
+    if x2.stride(1) != 1:
+        x2 = x2.contiguous()
+    M = x2.shape[0]
+    out_dtype = torch.float32 if epilogue == EPI_RESID_GATE_F32 else torch.bfloat16
+    if out is None:
+        out = torch.empty((M, N), dtype=out_dtype, device=x.device)
+    o2 = out.reshape(M, N)
+    assert o2.dtype == out_dtype and o2.stride(1) == 1
+    r2 = None
+    if resid is not None:
+        _require_cuda_bf16(resid, "resid")
+        r2 = resid.reshape(M, N)
+        assert r2.stride(1) == 1
+    if bias is not None:
+        _require_cuda_bf16(bias, "bias")
+        assert bias.is_contiguous() and bias.numel() == N
+    linear_sp(x2, M, K, x2.stride(0), w, bias, o2, o2.stride(0), epilogue, resid=r2, gate=gate, gate_rows=gate_rows)
+    return out.reshape(*x.shape[:-1], N)
 
 
 def _check_grouped(t, D: int, rows: int, M: int, name: str) -> int:
@@ -168,10 +252,19 @@ def _check_grouped(t, D: int, rows: int, M: int, name: str) -> int:
 def linear_sp(x: torch.Tensor, M: int, K: int, ldx: int, w: torch.Tensor, bias, out: torch.Tensor, ldo: int,
               epilogue: int = EPI_BIAS, x_seg_len: int = 0, x_seg_stride: int = 0, out_col_offsets=None, resid=None,
               gate=None, gate_rows: int = 0) -> None:
-    """fvb_linear_bf16_sp on raw buffers (x / out are base tensors; the logical shapes are given explicitly)."""
+    """fvb_linear_bf16_sp on raw buffers (x / out are base tensors; the logical shapes are given explicitly);
+    fvb_linear_w8_sp, with the same arguments, when w is an Int8Weight."""
     N = w.shape[0]
     ldr = resid.stride(0) if resid is not None else 0
     gate_stride = _check_grouped(gate, N, gate_rows, M, "gate")
+    if isinstance(w, Int8Weight):
+        if not x.is_cuda or w.q.device != x.device:
+            raise FvbError("x and the Int8Weight must be on the same CUDA device")
+        check(lib().fvb_linear_w8_sp(ptr(x), c_int64(ldx), c_int(x_seg_len), c_int64(x_seg_stride), ptr(w.q),
+                                     c_int64(w.q.stride(0)), _f32p(w.scale), ptr(bias), ptr(out), c_int64(ldo),
+                                     ptr(out_col_offsets), ptr(resid), c_int64(ldr), _f32p(gate), c_int(gate_rows),
+                                     c_int64(gate_stride), c_int(M), c_int(N), c_int(K), c_int(epilogue), stream_ptr()))
+        return
     check(lib().fvb_linear_bf16_sp(ptr(x), c_int64(ldx), c_int(x_seg_len), c_int64(x_seg_stride), ptr(w), c_int64(w.stride(0)),
                                    ptr(bias), ptr(out), c_int64(ldo), ptr(out_col_offsets), ptr(resid), c_int64(ldr),
                                    cast(ptr(gate), POINTER(c_float)), c_int(gate_rows), c_int64(gate_stride), c_int(M), c_int(N),

@@ -27,6 +27,9 @@ What install() registers, and the reference interface each piece stands behind:
   linear (FP8)        @register_quantization_config("fvb200_fp8") Fvb200Fp8Config: Fvb200Fp8LinearMethod loads the same
                       bf16 weight, quantises it to e4m3 per output channel in process_weights_after_loading (the bf16
                       parameter is replaced, not kept) and applies ops.linear_fp8 (activations quantised per token).
+  linear (INT8 w)     @register_quantization_config("fvb200_int8w") Fvb200Int8WeightConfig: Fvb200Int8WeightLinearMethod
+                      loads the same bf16 weight, quantises it to int8 per output channel in process_weights_after_loading
+                      (the bf16 parameter is replaced) and applies ops.linear_any (bf16 activations, fvb_linear_w8_sp).
   custom ops          RMSNorm.forward_cuda (fastvideo/layers/layernorm.py:12-83) on fvb_rmsnorm_rope, and
                       CustomOp.dispatch_forward (fastvideo/layers/custom_op.py:53-57, hard-wired to forward_native) routed
                       to forward_cuda for the classes that got one.
@@ -50,6 +53,7 @@ DENSE_BACKEND_NAME = "FVB200_ATTN"
 DENSE_8BIT_BACKEND_NAME = "FVB200_ATTN_8BIT"
 QUANT_NAME = "fvb200_bf16"
 QUANT_NAME_FP8 = "fvb200_fp8"
+QUANT_NAME_INT8W = "fvb200_int8w"
 
 _state: types.SimpleNamespace | None = None
 
@@ -286,6 +290,40 @@ def _define():
         def get_quant_method(self, layer, prefix: str):
             return Fvb200Fp8LinearMethod() if isinstance(layer, LinearBase) else None
 
+    class Fvb200Int8WeightLinearMethod(Fvb200LinearMethod):
+        """Same bf16 weight parameter as Fvb200LinearMethod; after loading it becomes `weight` (int8 [N, K]) plus
+        `weight_scale` (fp32 [N]), and apply() runs fvb_linear_w8_sp on the bf16 activations."""
+
+        def process_weights_after_loading(self, layer) -> None:
+            w = layer.weight
+            if not w.is_cuda:
+                raise FvbError("fvb200_int8w quantises its weights on the GPU: load the model onto a CUDA device")
+            iw = ops.Int8Weight.quantize(w.data)
+            layer.weight = Parameter(iw.q, requires_grad=False)  # drops the bf16 parameter
+            layer.weight_scale = Parameter(iw.scale, requires_grad=False)
+
+        def apply(self, layer, x, bias=None):
+            if not x.is_cuda:
+                raise FvbError("fvb200_int8w linear needs CUDA tensors (there is no CPU fallback)")
+            if layer.weight.dtype != torch.int8:
+                raise FvbError("fvb200_int8w linear: weights are not quantised (process_weights_after_loading did not run)")
+            if x.dtype != torch.bfloat16:
+                raise FvbError(f"fvb200_int8w linear takes bf16 activations (got {x.dtype})")
+            w = ops.Int8Weight(layer.weight, layer.weight_scale)
+            b = None if bias is None else bias.to(torch.bfloat16)
+            return ops.linear_any(x, w, b)
+
+    class Fvb200Int8WeightConfig(Fvb200Bf16Config):
+        def get_name(self):
+            return QUANT_NAME_INT8W
+
+        @classmethod
+        def get_min_capability(cls) -> int:
+            return 90  # sm_90a wgmma GEMM
+
+        def get_quant_method(self, layer, prefix: str):
+            return Fvb200Int8WeightLinearMethod() if isinstance(layer, LinearBase) else None
+
     ns.__dict__.update(
         Fvb200AttentionMetadata=Fvb200AttentionMetadata, Fvb200AttentionMetadataBuilder=Fvb200AttentionMetadataBuilder,
         Fvb200AttentionImpl=Fvb200AttentionImpl, Fvb200AttentionBackend=Fvb200AttentionBackend,
@@ -293,7 +331,8 @@ def _define():
         Fvb200VideoSparseAttentionMetadata=Fvb200VideoSparseAttentionMetadata,
         Fvb200VideoSparseAttentionMetadataBuilder=Fvb200VideoSparseAttentionMetadataBuilder,
         Fvb200VideoSparseAttentionImpl=Fvb200VideoSparseAttentionImpl, Fvb200LinearMethod=Fvb200LinearMethod,
-        Fvb200Bf16Config=Fvb200Bf16Config, Fvb200Fp8LinearMethod=Fvb200Fp8LinearMethod, Fvb200Fp8Config=Fvb200Fp8Config)
+        Fvb200Bf16Config=Fvb200Bf16Config, Fvb200Fp8LinearMethod=Fvb200Fp8LinearMethod, Fvb200Fp8Config=Fvb200Fp8Config,
+        Fvb200Int8WeightLinearMethod=Fvb200Int8WeightLinearMethod, Fvb200Int8WeightConfig=Fvb200Int8WeightConfig)
     return ns
 
 
@@ -425,6 +464,8 @@ def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, c
             Q.register_quantization_config(QUANT_NAME)(ns.Fvb200Bf16Config)
         if QUANT_NAME_FP8 not in Q.QUANTIZATION_METHODS:
             Q.register_quantization_config(QUANT_NAME_FP8)(ns.Fvb200Fp8Config)
+        if QUANT_NAME_INT8W not in Q.QUANTIZATION_METHODS:
+            Q.register_quantization_config(QUANT_NAME_INT8W)(ns.Fvb200Int8WeightConfig)
 
     if custom_ops:
         from fastvideo.layers.custom_op import CustomOp
@@ -455,4 +496,5 @@ def uninstall() -> None:
 
 
 __all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "route_dense", "DENSE_BACKEND_NAME",
-           "DENSE_8BIT_BACKEND_NAME", "QUANT_NAME", "QUANT_NAME_FP8"]
+           "DENSE_8BIT_BACKEND_NAME", "QUANT_NAME", "QUANT_NAME_FP8",
+           "QUANT_NAME_INT8W"]

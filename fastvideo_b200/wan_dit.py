@@ -52,6 +52,15 @@ class WanDiTConfig:
     # Opt-in 8-bit self-attention (INT8 Q K^T, FP8 P V; ops.quantize_attention_8bit + ops.attention_8bit), dense and the VSA
     # sparse branch. Cross-attention and the VSA compression branch stay bf16. Independent of fp8_linears.
     attention_8bit: bool = False
+    # Opt-in INT8 weights: every block linear (INT8_LINEARS) keeps int8 weights with one fp32 scale per output channel
+    # (ops.Int8Weight, quantised once at load; no bf16 copy is kept) and runs on bf16 activations through
+    # fvb_linear_w8_sp. The embedders, patch embedding and proj_out stay bf16. Combines with vsa and attention_8bit, and
+    # runs on the sequence-parallel and causal paths; exclusive with fp8_linears.
+    int8_weights: bool = False
+
+    def __post_init__(self):
+        if self.int8_weights and self.fp8_linears:
+            raise ops.FvbError("int8_weights and fp8_linears are exclusive: pick one weight format")
 
     @property
     def head_dim(self) -> int:
@@ -108,6 +117,8 @@ def random_state_dict(cfg: WanDiTConfig, device="cuda", seed: int = 2029, dtype=
 
 # WanBlock weights that multiply the token stream; with WanDiTConfig.fp8_linears they are ops.Fp8Weight
 FP8_LINEARS = ("w_qkv", "w_o", "w_q2", "w_o2", "w_1", "w_2")
+# every WanBlock linear weight; with WanDiTConfig.int8_weights they are ops.Int8Weight (w_kv_img only on I2V blocks)
+INT8_LINEARS = FP8_LINEARS + ("w_kv2", "w_kv_img")
 
 
 class WanBlock:
@@ -145,6 +156,10 @@ class WanBlock:
         if cfg.fp8_linears:
             for n in FP8_LINEARS:  # replacing the attribute drops the block's bf16 copy
                 setattr(self, n, ops.Fp8Weight.quantize(getattr(self, n)))
+        if cfg.int8_weights:
+            for n in INT8_LINEARS:
+                if getattr(self, n) is not None:
+                    setattr(self, n, ops.Int8Weight.quantize(getattr(self, n)))
 
 
 @dataclass
@@ -195,12 +210,12 @@ def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: Wan
     img = None
     if blk.w_kv_img is not None:
         ctx_img, ctx = ctx[:I2V_IMAGE_TOKENS], ctx[I2V_IMAGE_TOKENS:]
-        kvi = ops.linear(ctx_img.contiguous(), blk.w_kv_img, blk.b_kv_img)
+        kvi = ops.linear_any(ctx_img.contiguous(), blk.w_kv_img, blk.b_kv_img)
         ops.rmsnorm_rope_(kvi[:, :D], blk.norm_k_img, head_dim=d, eps=cfg.eps)
         img = ops.attention(hd(q2), hd(kvi[:, :D]), hd(kvi[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
         if ctx.shape[0] == 0:
             return img  # zeros_like(q) + img_x
-    kv2 = ops.linear(ctx.contiguous(), blk.w_kv2, blk.b_kv2)  # [L, 2D]
+    kv2 = ops.linear_any(ctx.contiguous(), blk.w_kv2, blk.b_kv2)  # [L, 2D]
     ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
     a2 = ops.attention(hd(q2), hd(kv2[:, :D]), hd(kv2[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
     return a2 if img is None else a2 + img  # `x = x + img_x` on bf16 tensors
@@ -276,7 +291,8 @@ class WanDiT:
     @classmethod
     def random(cls, cfg: WanDiTConfig, device="cuda", seed: int = 2029) -> "WanDiT":
         """Synthetic random-init model of the given architecture, built layer by layer so that peak memory stays
-        at one copy of the weights (30 GB for a 14B expert in bf16; with fp8_linears the block weights take half)."""
+        at one copy of the weights (30 GB for a 14B expert in bf16; with fp8_linears or int8_weights the block weights take
+        half)."""
         blocks = []
         for i in range(cfg.num_layers):
             one = WanDiTConfig(**{**cfg.__dict__, "num_layers": 1})

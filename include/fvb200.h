@@ -107,6 +107,26 @@ int fvb_linear_fp8(const void* xq, int64_t ldx, const float* x_scale, const void
                    const void* bias, void* out, int64_t ldo, const void* resid, int64_t ldr, const float* gate, int gate_rows,
                    int64_t gate_stride, int M, int N, int K, int epilogue, void* stream);
 
+/* --------------------------------------------------------------------------------------------
+ * INT8 weight-only linear layers: bf16 activations x per-output-channel int8 weights
+ *
+ * fvb_linear_w8_sp: x bf16 [M, K] (ld=ldx, or segmented by x_seg_len / x_seg_stride as in fvb_linear_bf16_sp);
+ *   wq int8 [N, K] ld=ldw (a multiple of 16: 16-byte rows) with w_scale fp32 [N]:
+ *   acc[m, n] = sum_k x[m, k] * wq[n, k]   (every bf16 x int8 product is exact in fp32; int8 -> bf16 is exact, so the
+ *                                           accumulation is the bf16 GEMM's)
+ *   y = bf16((acc * w_scale[n]) + bias[n])  (fp32 round-to-nearest, in that order, no contraction; bias may be NULL)
+ *   then the epilogue exactly as in fvb_linear_bf16: FVB_EPI_BIAS, BIAS_GELU_TANH, RESID_GATE_F32, RESID_GATE_BF16,
+ *   RESID_GATE_BF16R, RESID_BF16, with the same gate / gate_rows grouping. out_col_offsets, x_seg_len, x_seg_stride and
+ *   every other argument follow the rules of fvb_linear_bf16_sp; x_seg_len = 0 with out_col_offsets = NULL is the plain
+ *   linear. K tails (K not a multiple of 64) are zero-filled on load.
+ * The weights are typically quantised once at load: scale[n] = amax_n / 127, wq[n, k] = clamp(rint(w[n, k] * (127 /
+ * amax_n)), -127, 127); an all-zero row has scale 1 and wq = 0.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_linear_w8_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_stride, const void* wq, int64_t ldw,
+                     const float* w_scale, const void* bias, void* out, int64_t ldo, const int64_t* out_col_offsets,
+                     const void* resid, int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M, int N,
+                     int K, int epilogue, void* stream);
+
 /* Batched C[i] = bf16(A[i] @ B[i]^T), optionally followed by out = bf16(float(C) / div) (div = 0 or 1: none).
  * A[i]: [M, K] ld=lda, B[i]: [N, K] ld=ldb, out[i]: [M, N] ld=ldo; batch strides in elements (multiples of 8).
  * Replaces the block-level matmuls of video_sparse_attn's compression branch
