@@ -1,7 +1,8 @@
-// gemm_sm90.cu -- persistent, warp-specialised GEMM for sm_90a, bf16, fp8 (e4m3) or int8-weight operands:
+// gemm_sm90.cu -- persistent, warp-specialised GEMM for sm_90a, bf16, fp8 (e4m3), int8-weight or int8 x int8 operands:
 //   out = epilogue(x[M,K] @ w[N,K]^T + bias)                                   (bf16)
 //   out = epilogue((x_q[M,K] @ w_q[N,K]^T) * x_scale[m] * w_scale[n] + bias)   (e4m3, per-row / per-channel scales)
 //   out = epilogue((x[M,K] @ w_q[N,K]^T) * w_scale[n] + bias)                  (bf16 x, int8 w, per-channel scales)
+//   out = epilogue((x_q[M,K] @ w_q[N,K]^T) * x_scale[m] * w_scale[n] + bias)   (int8 x and w, s32 accumulators)
 // TMA (128B swizzle) -> shared-memory ring -> wgmma (two warpgroups, 64 rows x BN each, fp32 accumulators in registers)
 // -> epilogue straight from the accumulator registers with fused bias / GELU(tanh) / gated residual.
 // A k-block is one 128-byte swizzle row of both operands: 64 bf16 or 128 e4m3 elements, so a stage holds the same bytes
@@ -10,6 +11,9 @@
 // The int8-weight path (W8) runs the bf16 MMAs: each k-block's BN x 64 int8 weight tile lands, unswizzled, in the second
 // half of the stage's bf16 B region, and warps 1-3 of the producer warpgroup widen it in place to the 128B-swizzled
 // bf16 tile the B descriptor reads. int8 -> bf16 is exact, so the products are those of a bf16 GEMM on integer weights.
+// The int8 x int8 path (I8, W8A8) loads both operands like the fp8 path (128-element k-blocks, 128B swizzle) and runs
+// s8 MMAs into s32 accumulators. |acc| <= 127^2 K fits in s32 for K <= FVB_I8_MAX_K, so the sums are exact and need no
+// promotion registers: the tile widths and the one-k-block-in-flight mainloop are the bf16 path's.
 //
 // Stands behind fastvideo/layers/linear.py:146-156 (F.linear) and the elementwise op that follows
 // each linear in fastvideo/models/dits/wanvideo.py:394-431; rounding points mirror the reference's
@@ -30,7 +34,8 @@ namespace fvb {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;   // 64 bf16 = one 128B swizzle row
-constexpr int GEMM_BK_FP8 = 128;  // 128 e4m3 = one 128B swizzle row
+constexpr int GEMM_BK_FP8 = 128;  // 128 e4m3 / int8 = one 128B swizzle row
+constexpr int FVB_I8_MAX_K = 133144;  // 127^2 * 133144 < 2^31
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_GROUP_M = 8;
 
@@ -52,8 +57,8 @@ struct GemmParams {
   int stripe_n;  // > 0: weight-stripe raster with this many column tiles per stripe (see tile_coords)
 };
 
-// e4m3 / int8-weight operands: the per-row / per-channel scales (a_scale: e4m3 only). The bf16 kernels keep taking the
-// plain GemmParams.
+// e4m3 / int8 operands: the per-row / per-channel scales (a_scale: e4m3 and int8 x int8 only). The bf16 kernels keep
+// taking the plain GemmParams.
 struct GemmParamsFp8 : GemmParams {
   const float* a_scale;  // [M]
   const float* b_scale;  // [N_valid]
@@ -162,12 +167,16 @@ FVB_DEVICE void w8_widen_tile(uint32_t sb, int t) {
   }
 }
 
-// FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); neither: bf16 x bf16
-template <int BN, int EPI, bool FP8, bool W8 = false>
+FVB_DEVICE float acc_f32(float v) { return v; }
+FVB_DEVICE float acc_f32(int32_t v) { return __int2float_rn(v); }
+
+// FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); I8: int8 x int8 (W8A8); none: bf16 x bf16
+template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8 || W8> p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8 || W8 || I8> p) {
   using Cfg = GemmCfg<BN>;
-  constexpr int BK = FP8 ? GEMM_BK_FP8 : GEMM_BK;
+  constexpr int BK = FP8 || I8 ? GEMM_BK_FP8 : GEMM_BK;
+  using Acc = std::conditional_t<I8, int32_t, float>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
@@ -267,9 +276,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     int m_blk, n_blk;
     const int bt = tile / tiles_per_batch;
     tile_coords(tile - bt * tiles_per_batch, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
-    float acc[BN / 2];
+    Acc acc[BN / 2];
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = Acc(0);
     int prev = -1;
     if constexpr (FP8) {
       // per k-block partial sums in `part` (the first MMA overwrites it), promoted into the fp32 accumulators after the
@@ -305,8 +314,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const uint64_t da = make_desc_kmajor_sw128(sa);
       const uint64_t db = make_desc_kmajor_sw128(sb);
       wgmma_fence();
+      if constexpr (I8) {
 #pragma unroll
-      for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k));
+        for (int k = 0; k < GEMM_BK_FP8 / 32; ++k) wgmma_ss_s8<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), 1);
+      } else {
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k));
+      }
       wgmma_commit();
       // keep one k-block of MMAs in flight: the stage read by the previous group is free once it completes
       wgmma_wait<1>();
@@ -329,7 +343,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (p.gate_rows > 0)
         for (int i = 0; i < 2; ++i) gate_rows_p[i] += int64_t((row0 + 8 * i) / p.gate_rows) * p.gate_stride;
     float sx[2] = {1.f, 1.f};
-    if constexpr (FP8)
+    if constexpr (FP8 || I8)
       for (int i = 0; i < 2; ++i) sx[i] = row0 + 8 * i < p.M ? __ldg(p.a_scale + row0 + 8 * i) : 0.f;
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
@@ -339,7 +353,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       float2 bf = make_float2(0.f, 0.f);
       if (p.bias != nullptr) bf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
       float2 sw = make_float2(1.f, 1.f);
-      if constexpr (FP8 || W8) {
+      if constexpr (FP8 || W8 || I8) {
         sw.x = col < p.N_valid ? __ldg(p.b_scale + col) : 0.f;
         sw.y = col + 1 < p.N_valid ? __ldg(p.b_scale + col + 1) : 0.f;
       }
@@ -347,8 +361,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       for (int i = 0; i < 2; ++i) {
         const int row = row0 + 8 * i;
         if (row >= p.M) continue;
-        float f0 = acc[4 * j + 2 * i], f1 = acc[4 * j + 2 * i + 1];
-        if constexpr (FP8) {  // (acc * s_x[m]) * s_w[n], fp32 round-to-nearest, before the bias
+        // I8: float(acc) rounds to nearest (exact up to 2^24)
+        float f0 = acc_f32(acc[4 * j + 2 * i]), f1 = acc_f32(acc[4 * j + 2 * i + 1]);
+        if constexpr (FP8 || I8) {  // (acc * s_x[m]) * s_w[n], fp32 round-to-nearest, before the bias
           f0 = __fmul_rn(__fmul_rn(f0, sx[i]), sw.x);
           f1 = __fmul_rn(__fmul_rn(f1, sx[i]), sw.y);
         } else if constexpr (W8) {  // acc * s_w[n], fp32 round-to-nearest, before the bias
@@ -399,10 +414,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
-template <int BN, int EPI, bool FP8, bool W8 = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8 || W8>& p, cudaStream_t st) {
+template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8 || W8 || I8>& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_kernel<BN, EPI, FP8, W8>;
+  auto kern = gemm_kernel<BN, EPI, FP8, W8, I8>;
   static bool configured = false;
   if (!configured) {
     FVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -430,18 +445,18 @@ static int dispatch_epi(int epi, const CUtensorMap& a, const CUtensorMap& b, con
   return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue%s");
 }
 
-// fp8 / int8-weight operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
-template <int BN, bool FP8, bool W8>
+// fp8 / int8 operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
+template <int BN, bool FP8, bool W8, bool I8 = false>
 static int dispatch_epi_scaled(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsFp8& p, cudaStream_t st) {
   switch (epi) {
-    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, FP8, W8>(a, b, p, st);
-    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, FP8, W8>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, FP8, W8>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, FP8, W8>(a, b, p, st);
-    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, FP8, W8>(a, b, p, st);
-    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, FP8, W8>(a, b, p, st);
+    case FVB_EPI_BIAS: return launch_gemm<BN, FVB_EPI_BIAS, FP8, W8, I8>(a, b, p, st);
+    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm<BN, FVB_EPI_BIAS_GELU_TANH, FP8, W8, I8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_F32: return launch_gemm<BN, FVB_EPI_RESID_GATE_F32, FP8, W8, I8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16, FP8, W8, I8>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm<BN, FVB_EPI_RESID_GATE_BF16R, FP8, W8, I8>(a, b, p, st);
+    case FVB_EPI_RESID_BF16: return launch_gemm<BN, FVB_EPI_RESID_BF16, FP8, W8, I8>(a, b, p, st);
   }
-  return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue for fvb_linear_fp8 / fvb_linear_w8_sp%s");
+  return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue for fvb_linear_fp8 / fvb_linear_w8_sp / fvb_linear_w8a8_sp%s");
 }
 
 }  // namespace fvb
@@ -452,17 +467,26 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
                      const void* bias, void* out, int64_t ldo, int64_t o_batch, const int64_t* out_col_offsets,
                      const void* resid, int64_t ldr,
                      const float* gate, int gate_rows, int64_t gate_stride, float div, int M, int N, int K, int batch,
-                     int epilogue, void* stream, const float* x_scale = nullptr, const float* w_scale = nullptr) {
-  // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales.
+                     int epilogue, void* stream, const float* x_scale = nullptr, const float* w_scale = nullptr,
+                     bool int8_operands = false) {
+  // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales, or
+  // int8 with the same scales when int8_operands is set.
   // w_scale alone: x is bf16 and w is int8 with per-output-channel fp32 scales.
-  const bool fp8 = x_scale != nullptr;
-  const bool w8 = !fp8 && w_scale != nullptr;
+  const bool i8 = x_scale != nullptr && int8_operands;
+  const bool fp8 = x_scale != nullptr && !i8;
+  const bool w8 = x_scale == nullptr && w_scale != nullptr;
   FVB_CHECK_ARG(x && w && out, "null pointer");
   FVB_CHECK_ARG(M > 0 && N > 0 && K > 0 && batch > 0, "empty problem");
   if (fp8) {
     FVB_CHECK_ARG(w_scale != nullptr, "w_scale required");
     FVB_CHECK_ARG(batch == 1 && a_seg_len <= 0 && out_col_offsets == nullptr, "fp8 operands: plain row-major, unbatched");
     FVB_CHECK_ARG(ldx % 16 == 0 && ldw % 16 == 0, "fp8 ldx/ldw must be multiples of 16 (16-byte rows)");
+  }
+  if (i8) {
+    FVB_CHECK_ARG(w_scale != nullptr, "w_scale required");
+    FVB_CHECK_ARG(batch == 1 && a_seg_len <= 0, "int8 operands: plain row-major, unbatched");
+    FVB_CHECK_ARG(ldx % 16 == 0 && ldw % 16 == 0, "int8 ldx/ldw must be multiples of 16 (16-byte rows)");
+    FVB_CHECK_ARG(K <= FVB_I8_MAX_K, "int8 operands: K > 133144 could overflow the s32 accumulator");
   }
   if (w8) {
     FVB_CHECK_ARG(batch == 1, "int8 weights: unbatched");
@@ -489,9 +513,9 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
   // fp8: the promotion registers double the accumulator footprint, so 128 columns is the widest tile that fits
   const int BN = fp8 ? (N >= 128 ? 128 : 64)
                      : (N >= 256 && N % 256 == 0) ? 256 : (N >= 128 && N % 128 == 0 ? 128 : (N >= 192 ? 256 : 64));
-  const int BK = fp8 ? GEMM_BK_FP8 : GEMM_BK;
-  const int esz = fp8 ? 1 : 2;  // operand element bytes
-  const int wsz = fp8 || w8 ? 1 : 2;
+  const int BK = fp8 || i8 ? GEMM_BK_FP8 : GEMM_BK;
+  const int esz = fp8 || i8 ? 1 : 2;  // operand element bytes
+  const int wsz = fp8 || w8 || i8 ? 1 : 2;
 
   CUtensorMap tmA, tmB;
   if (a_seg_len <= 0 || a_seg_len >= K) {
@@ -505,7 +529,7 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     uint64_t str[4] = {(uint64_t)esz, (uint64_t)ldx * esz, (uint64_t)a_seg_stride * esz,
                        batch > 1 ? (uint64_t)x_batch * esz : 16};  // unused dimension (size 1): any 16-byte multiple
     uint32_t box[4] = {(uint32_t)BK, GEMM_BM, 1, 1};
-    int r = fp8 ? make_tmap_u8(&tmA, x, 4, dims, str, box) : make_tmap_bf16(&tmA, x, 4, dims, str, box);
+    int r = fp8 || i8 ? make_tmap_u8(&tmA, x, 4, dims, str, box) : make_tmap_bf16(&tmA, x, 4, dims, str, box);
     if (r) return r;
   }
   {
@@ -513,7 +537,7 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     uint64_t str[3] = {(uint64_t)wsz, (uint64_t)ldw * wsz, (uint64_t)(batch > 1 ? w_batch : ldw * (int64_t)N) * wsz};
     uint32_t box[3] = {(uint32_t)BK, (uint32_t)BN, 1};
     // int8 weights land unswizzled in a staging area and are widened into the swizzled bf16 layout in shared memory
-    int r = fp8  ? make_tmap_u8(&tmB, w, 3, dims, str, box)
+    int r = fp8 || i8 ? make_tmap_u8(&tmB, w, 3, dims, str, box)
             : w8 ? make_tmap_u8(&tmB, w, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE)
                  : make_tmap_bf16(&tmB, w, 3, dims, str, box);
     if (r) return r;
@@ -553,6 +577,11 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
   if (fp8)
     return BN == 128 ? dispatch_epi_scaled<128, true, false>(epilogue, tmA, tmB, p, st)
                      : dispatch_epi_scaled<64, true, false>(epilogue, tmA, tmB, p, st);
+  if (i8) {
+    if (BN == 256) return dispatch_epi_scaled<256, false, false, true>(epilogue, tmA, tmB, p, st);
+    if (BN == 128) return dispatch_epi_scaled<128, false, false, true>(epilogue, tmA, tmB, p, st);
+    return dispatch_epi_scaled<64, false, false, true>(epilogue, tmA, tmB, p, st);
+  }
   if (w8) {
     if (BN == 256) return dispatch_epi_scaled<256, false, true>(epilogue, tmA, tmB, p, st);
     if (BN == 128) return dispatch_epi_scaled<128, false, true>(epilogue, tmA, tmB, p, st);
@@ -611,4 +640,14 @@ extern "C" int fvb_linear_w8_sp(const void* x, int64_t ldx, int x_seg_len, int64
   if (out_col_offsets != nullptr && N % 128 != 0) return set_error(FVB_ERR_INVALID_ARG, "column-block offsets need N %% 128 == 0%s");
   return gemm_impl(x, ldx, 0, x_seg_len, x_seg_stride, wq, ldw, 0, bias, out, ldo, 0, out_col_offsets, resid, ldr, gate,
                    gate_rows, gate_stride, 1.0f, M, N, K, 1, epilogue, stream, nullptr, w_scale);
+}
+
+extern "C" int fvb_linear_w8a8_sp(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw,
+                                  const float* w_scale, const void* bias, void* out, int64_t ldo, const int64_t* out_col_offsets,
+                                  const void* resid, int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M,
+                                  int N, int K, int epilogue, void* stream) {
+  if (x_scale == nullptr || w_scale == nullptr) return set_error(FVB_ERR_INVALID_ARG, "invalid argument: x_scale and w_scale are required%s");
+  if (out_col_offsets != nullptr && N % 128 != 0) return set_error(FVB_ERR_INVALID_ARG, "column-block offsets need N %% 128 == 0%s");
+  return gemm_impl(xq, ldx, 0, 0, 0, wq, ldw, 0, bias, out, ldo, 0, out_col_offsets, resid, ldr, gate, gate_rows, gate_stride,
+                   1.0f, M, N, K, 1, epilogue, stream, x_scale, w_scale, true);
 }

@@ -145,11 +145,35 @@ def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: torch.Tensor | None = None, 
     return out.reshape(*x.shape[:-1], N)
 
 
-class Int8Weight:
-    """A linear weight w[N, K] held as int8 rows with one fp32 scale per output channel (w ~= q * scale[:, None]); the
-    activations it multiplies stay bf16 (fvb_linear_w8_sp)."""
+def quantize_int8_rows(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """fvb_quantize_int8_rows: bf16 [M, K] (rows may be strided; K % 8 == 0) -> (q int8 [M, K], scale fp32 [M]) with
+    x[r] ~= q[r] * scale[r], by the rule of Int8Weight.quantize. q's row stride is K rounded up to 16 (16-byte rows, what
+    fvb_linear_w8a8_sp loads)."""
+    _require_cuda_bf16(x, "x")
+    if x.dim() != 2 or x.stride(1) != 1:
+        raise FvbError("x must be a 2-D view with unit inner stride")
+    M, K = x.shape
+    return _quantize_int8_rows_sp(x, M, K, x.stride(0))
 
-    def __init__(self, q: torch.Tensor, scale: torch.Tensor):
+
+def _quantize_int8_rows_sp(x: torch.Tensor, M: int, K: int, ldx: int, x_seg_len: int = 0, x_seg_stride: int = 0):
+    """quantize_int8_rows on a raw buffer with linear_sp's geometry (x_seg_len / x_seg_stride: fvb_linear_bf16_sp's K
+    segmentation); each row comes out contiguous."""
+    _require_cuda_bf16(x, "x")
+    ldq = (K + 15) // 16 * 16
+    q = torch.empty((M, ldq), dtype=torch.int8, device=x.device)
+    scale = torch.empty((M,), dtype=torch.float32, device=x.device)
+    check(lib().fvb_quantize_int8_rows(ptr(x), c_int64(ldx), c_int(x_seg_len), c_int64(x_seg_stride), c_int(M), c_int(K),
+                                       ptr(q), c_int64(ldq), _f32p(scale), stream_ptr()))
+    return q[:, :K], scale
+
+
+class Int8Weight:
+    """A linear weight w[N, K] held as int8 rows with one fp32 scale per output channel (w ~= q * scale[:, None]). The
+    activations it multiplies stay bf16 (fvb_linear_w8_sp), or, with int8_activations, are quantised to int8 with one
+    scale per token (quantize_int8_rows) and multiplied on the s8 tensor cores (fvb_linear_w8a8_sp)."""
+
+    def __init__(self, q: torch.Tensor, scale: torch.Tensor, int8_activations: bool = False):
         if q.dtype != torch.int8 or q.dim() != 2 or q.stride(1) != 1 or q.stride(0) % 16 != 0:
             raise FvbError("Int8Weight.q must be int8 [N, K] with 16-byte-aligned rows")
         if scale.dtype != torch.float32 or scale.shape != (q.shape[0],) or not scale.is_contiguous():
@@ -157,9 +181,10 @@ class Int8Weight:
         if q.device != scale.device:
             raise FvbError("Int8Weight.q and scale must be on the same device")
         self.q, self.scale = q, scale
+        self.int8_activations = bool(int8_activations)
 
     @classmethod
-    def quantize(cls, w: torch.Tensor) -> "Int8Weight":
+    def quantize(cls, w: torch.Tensor, int8_activations: bool = False) -> "Int8Weight":
         """[N, K] -> per-output-channel int8, once at load (torch, on w's device): amax = max|w[n]| (fp32),
         scale = amax / 127, q = clamp(rint(w * (127 / amax)), -127, 127); an all-zero row gets scale 1 and q = 0."""
         if w.dim() != 2:
@@ -174,13 +199,13 @@ class Int8Weight:
         ld = (K + 15) // 16 * 16
         q = torch.zeros((N, ld), dtype=torch.int8, device=w.device)
         q[:, :K] = torch.clamp(torch.round(w32 * inv[:, None]), -127, 127).to(torch.int8)
-        return cls(q[:, :K], scale.contiguous())
+        return cls(q[:, :K], scale.contiguous(), int8_activations)
 
     def __getitem__(self, rows) -> "Int8Weight":
-        """Row slice w[a:b] (q rows and scale rows), e.g. the Q / K / V parts of a fused QKV weight."""
+        """Row slice w[a:b] (q rows and scale rows, same activation mode), e.g. the Q / K / V parts of a fused QKV weight."""
         if not isinstance(rows, slice) or rows.step not in (None, 1):
             raise FvbError("Int8Weight supports contiguous row slices only")
-        return Int8Weight(self.q[rows], self.scale[rows])
+        return Int8Weight(self.q[rows], self.scale[rows], self.int8_activations)
 
     @property
     def shape(self):
@@ -202,8 +227,8 @@ class Int8Weight:
 def linear_any(x: torch.Tensor, w, bias: torch.Tensor | None = None, epilogue: int = EPI_BIAS,
                resid: torch.Tensor | None = None, gate: torch.Tensor | None = None,
                out: torch.Tensor | None = None, gate_rows: int = 0) -> torch.Tensor:
-    """`linear` for whatever the weight holds: linear_fp8 for an Fp8Weight, fvb_linear_w8_sp for an Int8Weight,
-    `linear` for a bf16 tensor."""
+    """`linear` for whatever the weight holds: linear_fp8 for an Fp8Weight, fvb_linear_w8_sp for an Int8Weight
+    (fvb_quantize_int8_rows + fvb_linear_w8a8_sp when it is marked int8_activations), `linear` for a bf16 tensor."""
     if isinstance(w, Fp8Weight):
         return linear_fp8(x, w, bias, epilogue, resid, gate, out, gate_rows)
     if not isinstance(w, Int8Weight):
@@ -253,13 +278,21 @@ def linear_sp(x: torch.Tensor, M: int, K: int, ldx: int, w: torch.Tensor, bias, 
               epilogue: int = EPI_BIAS, x_seg_len: int = 0, x_seg_stride: int = 0, out_col_offsets=None, resid=None,
               gate=None, gate_rows: int = 0) -> None:
     """fvb_linear_bf16_sp on raw buffers (x / out are base tensors; the logical shapes are given explicitly);
-    fvb_linear_w8_sp, with the same arguments, when w is an Int8Weight."""
+    fvb_linear_w8_sp, with the same arguments, when w is an Int8Weight; when that weight is marked int8_activations, x
+    (segmented or not) is quantised to contiguous int8 rows first and fvb_linear_w8a8_sp runs on them."""
     N = w.shape[0]
     ldr = resid.stride(0) if resid is not None else 0
     gate_stride = _check_grouped(gate, N, gate_rows, M, "gate")
     if isinstance(w, Int8Weight):
         if not x.is_cuda or w.q.device != x.device:
             raise FvbError("x and the Int8Weight must be on the same CUDA device")
+        if w.int8_activations:
+            xq, xs = _quantize_int8_rows_sp(x, M, K, ldx, x_seg_len, x_seg_stride)
+            check(lib().fvb_linear_w8a8_sp(ptr(xq), c_int64(xq.stride(0)), _f32p(xs), ptr(w.q), c_int64(w.q.stride(0)),
+                                           _f32p(w.scale), ptr(bias), ptr(out), c_int64(ldo), ptr(out_col_offsets), ptr(resid),
+                                           c_int64(ldr), _f32p(gate), c_int(gate_rows), c_int64(gate_stride), c_int(M), c_int(N),
+                                           c_int(K), c_int(epilogue), stream_ptr()))
+            return
         check(lib().fvb_linear_w8_sp(ptr(x), c_int64(ldx), c_int(x_seg_len), c_int64(x_seg_stride), ptr(w.q),
                                      c_int64(w.q.stride(0)), _f32p(w.scale), ptr(bias), ptr(out), c_int64(ldo),
                                      ptr(out_col_offsets), ptr(resid), c_int64(ldr), _f32p(gate), c_int(gate_rows),

@@ -30,6 +30,9 @@ What install() registers, and the reference interface each piece stands behind:
   linear (INT8 w)     @register_quantization_config("fvb200_int8w") Fvb200Int8WeightConfig: Fvb200Int8WeightLinearMethod
                       loads the same bf16 weight, quantises it to int8 per output channel in process_weights_after_loading
                       (the bf16 parameter is replaced) and applies ops.linear_any (bf16 activations, fvb_linear_w8_sp).
+  linear (W8A8)       @register_quantization_config("fvb200_w8a8") Fvb200W8A8Config: Fvb200W8A8LinearMethod loads and
+                      quantises the weight like fvb200_int8w and applies ops.linear_any on an Int8Weight marked for int8
+                      activations (quantised per token by fvb_quantize_int8_rows, then fvb_linear_w8a8_sp).
   custom ops          RMSNorm.forward_cuda (fastvideo/layers/layernorm.py:12-83) on fvb_rmsnorm_rope, and
                       CustomOp.dispatch_forward (fastvideo/layers/custom_op.py:53-57, hard-wired to forward_native) routed
                       to forward_cuda for the classes that got one.
@@ -54,6 +57,7 @@ DENSE_8BIT_BACKEND_NAME = "FVB200_ATTN_8BIT"
 QUANT_NAME = "fvb200_bf16"
 QUANT_NAME_FP8 = "fvb200_fp8"
 QUANT_NAME_INT8W = "fvb200_int8w"
+QUANT_NAME_W8A8 = "fvb200_w8a8"
 
 _state: types.SimpleNamespace | None = None
 
@@ -293,6 +297,7 @@ def _define():
     class Fvb200Int8WeightLinearMethod(Fvb200LinearMethod):
         """Same bf16 weight parameter as Fvb200LinearMethod; after loading it becomes `weight` (int8 [N, K]) plus
         `weight_scale` (fp32 [N]), and apply() runs fvb_linear_w8_sp on the bf16 activations."""
+        int8_activations = False  # Fvb200W8A8LinearMethod: quantise the activations too
 
         def process_weights_after_loading(self, layer) -> None:
             w = layer.weight
@@ -309,7 +314,7 @@ def _define():
                 raise FvbError("fvb200_int8w linear: weights are not quantised (process_weights_after_loading did not run)")
             if x.dtype != torch.bfloat16:
                 raise FvbError(f"fvb200_int8w linear takes bf16 activations (got {x.dtype})")
-            w = ops.Int8Weight(layer.weight, layer.weight_scale)
+            w = ops.Int8Weight(layer.weight, layer.weight_scale, int8_activations=self.int8_activations)
             b = None if bias is None else bias.to(torch.bfloat16)
             return ops.linear_any(x, w, b)
 
@@ -324,6 +329,22 @@ def _define():
         def get_quant_method(self, layer, prefix: str):
             return Fvb200Int8WeightLinearMethod() if isinstance(layer, LinearBase) else None
 
+    class Fvb200W8A8LinearMethod(Fvb200Int8WeightLinearMethod):
+        """Fvb200Int8WeightLinearMethod whose apply() also quantises the bf16 activations to int8, one scale per token
+        (fvb_quantize_int8_rows), and runs fvb_linear_w8a8_sp."""
+        int8_activations = True
+
+    class Fvb200W8A8Config(Fvb200Bf16Config):
+        def get_name(self):
+            return QUANT_NAME_W8A8
+
+        @classmethod
+        def get_min_capability(cls) -> int:
+            return 90  # s8 wgmma: sm_90a
+
+        def get_quant_method(self, layer, prefix: str):
+            return Fvb200W8A8LinearMethod() if isinstance(layer, LinearBase) else None
+
     ns.__dict__.update(
         Fvb200AttentionMetadata=Fvb200AttentionMetadata, Fvb200AttentionMetadataBuilder=Fvb200AttentionMetadataBuilder,
         Fvb200AttentionImpl=Fvb200AttentionImpl, Fvb200AttentionBackend=Fvb200AttentionBackend,
@@ -332,7 +353,8 @@ def _define():
         Fvb200VideoSparseAttentionMetadataBuilder=Fvb200VideoSparseAttentionMetadataBuilder,
         Fvb200VideoSparseAttentionImpl=Fvb200VideoSparseAttentionImpl, Fvb200LinearMethod=Fvb200LinearMethod,
         Fvb200Bf16Config=Fvb200Bf16Config, Fvb200Fp8LinearMethod=Fvb200Fp8LinearMethod, Fvb200Fp8Config=Fvb200Fp8Config,
-        Fvb200Int8WeightLinearMethod=Fvb200Int8WeightLinearMethod, Fvb200Int8WeightConfig=Fvb200Int8WeightConfig)
+        Fvb200Int8WeightLinearMethod=Fvb200Int8WeightLinearMethod, Fvb200Int8WeightConfig=Fvb200Int8WeightConfig,
+        Fvb200W8A8LinearMethod=Fvb200W8A8LinearMethod, Fvb200W8A8Config=Fvb200W8A8Config)
     return ns
 
 
@@ -466,6 +488,8 @@ def install(dense: bool = True, vsa_backend: bool = True, linear: bool = True, c
             Q.register_quantization_config(QUANT_NAME_FP8)(ns.Fvb200Fp8Config)
         if QUANT_NAME_INT8W not in Q.QUANTIZATION_METHODS:
             Q.register_quantization_config(QUANT_NAME_INT8W)(ns.Fvb200Int8WeightConfig)
+        if QUANT_NAME_W8A8 not in Q.QUANTIZATION_METHODS:
+            Q.register_quantization_config(QUANT_NAME_W8A8)(ns.Fvb200W8A8Config)
 
     if custom_ops:
         from fastvideo.layers.custom_op import CustomOp

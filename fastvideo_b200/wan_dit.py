@@ -57,10 +57,16 @@ class WanDiTConfig:
     # fvb_linear_w8_sp. The embedders, patch embedding and proj_out stay bf16. Combines with vsa and attention_8bit, and
     # runs on the sequence-parallel and causal paths; exclusive with fp8_linears.
     int8_weights: bool = False
+    # Opt-in W8A8, on top of int8_weights: the activations of every INT8_LINEARS GEMM are quantised to int8 as well, one
+    # fp32 scale per token (fvb_quantize_int8_rows), and the GEMM runs s8 x s8 -> s32 (fvb_linear_w8a8_sp). Same paths as
+    # int8_weights; the weights are the same Int8Weight objects, marked for int8 activations.
+    int8_activations: bool = False
 
     def __post_init__(self):
         if self.int8_weights and self.fp8_linears:
             raise ops.FvbError("int8_weights and fp8_linears are exclusive: pick one weight format")
+        if self.int8_activations and not self.int8_weights:
+            raise ops.FvbError("int8_activations needs int8_weights=True (the W8A8 GEMM takes int8 weights)")
 
     @property
     def head_dim(self) -> int:
@@ -159,7 +165,7 @@ class WanBlock:
         if cfg.int8_weights:
             for n in INT8_LINEARS:
                 if getattr(self, n) is not None:
-                    setattr(self, n, ops.Int8Weight.quantize(getattr(self, n)))
+                    setattr(self, n, ops.Int8Weight.quantize(getattr(self, n), cfg.int8_activations))
 
 
 @dataclass

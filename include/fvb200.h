@@ -127,6 +127,37 @@ int fvb_linear_w8_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_st
                      const void* resid, int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M, int N,
                      int K, int epilogue, void* stream);
 
+/* --------------------------------------------------------------------------------------------
+ * W8A8 INT8 linear layers: per-token int8 activations x per-output-channel int8 weights
+ *
+ * fvb_quantize_int8_rows: x bf16 [M, K] (row stride ldx, a multiple of 8; K a multiple of 8), optionally segmented: with
+ *   0 < x_seg_len < K, element k of row r is x[r * ldx + (k / x_seg_len) * x_seg_stride + k % x_seg_len] (x_seg_len a
+ *   multiple of 8 dividing K, x_seg_stride a multiple of 8; the meaning of fvb_linear_bf16_sp). x_seg_len = 0: plain rows.
+ *   -> q int8 [M, K] (one contiguous row each, row stride ldq, a multiple of 8) and scale fp32 [M]:
+ *   amax = max_k |x[r, k]| (fp32, exact, over every segment of the row);
+ *   amax == 0: scale[r] = 1, q[r, :] = 0;
+ *   else inv = 127.0f / amax, q[r, k] = clamp(rint(x[r, k] * inv), -127, 127), scale[r] = amax / 127.0f
+ *   (IEEE round-to-nearest division and multiplication, rint half-to-even): the rule of the load-time weight quantiser.
+ *
+ * fvb_linear_w8a8_sp: xq int8 [M, K] ld=ldx with x_scale fp32 [M]; wq int8 [N, K] ld=ldw with w_scale fp32 [N]
+ *   (ldx, ldw multiples of 16: 16-byte rows):
+ *   acc[m, n] = sum_k xq[m, k] * wq[n, k]                          (s32, exact: K <= 133144 keeps 127^2 K below 2^31;
+ *                                                                   larger K is rejected)
+ *   y = bf16(((float(acc) * x_scale[m]) * w_scale[n]) + bias[n])   (float() and fp32 round-to-nearest, in that order, no
+ *                                                                   contraction; bias may be NULL)
+ *   then the epilogue exactly as in fvb_linear_bf16: FVB_EPI_BIAS, BIAS_GELU_TANH, RESID_GATE_F32, RESID_GATE_BF16,
+ *   RESID_GATE_BF16R, RESID_BF16, with the same gate / gate_rows grouping. out_col_offsets follows fvb_linear_bf16_sp
+ *   (N % 128 == 0); the A operand is never segmented (fvb_quantize_int8_rows gathers segmented rows). K tails (K not a
+ *   multiple of 128) are zero-filled on load.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_quantize_int8_rows(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_stride, int M, int K, void* q,
+                           int64_t ldq, float* scale, void* stream);
+
+int fvb_linear_w8a8_sp(const void* xq, int64_t ldx, const float* x_scale, const void* wq, int64_t ldw, const float* w_scale,
+                       const void* bias, void* out, int64_t ldo, const int64_t* out_col_offsets, const void* resid,
+                       int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, int M, int N, int K, int epilogue,
+                       void* stream);
+
 /* Batched C[i] = bf16(A[i] @ B[i]^T), optionally followed by out = bf16(float(C) / div) (div = 0 or 1: none).
  * A[i]: [M, K] ld=lda, B[i]: [N, K] ld=ldb, out[i]: [M, N] ld=ldo; batch strides in elements (multiples of 8).
  * Replaces the block-level matmuls of video_sparse_attn's compression branch
