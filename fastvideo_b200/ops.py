@@ -455,7 +455,12 @@ def attention_blocklist(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q2k_i
         # reference returns defined values there, so they are zero here (ADVICE r1: no uninitialised rows leave the API)
         alloc = torch.zeros if (q_off is None and q_len is not None) else torch.empty
         out = alloc((B, Sq, H, d), dtype=torch.bfloat16, device=q.device)
-    lse = torch.empty((B, H, Sq), dtype=torch.float32, device=q.device) if return_lse else None
+    lse = None
+    if return_lse:
+        # padded layout: rows past a tile's length are not computed; their LSE is that of a row without keys, -inf, so
+        # attention_blocklist_bwd gives them no weight
+        lse = (torch.full((B, H, Sq), float("-inf"), dtype=torch.float32, device=q.device) if (q_off is None and q_len is not None)
+               else torch.empty((B, H, Sq), dtype=torch.float32, device=q.device))
     assert q2k_idx.dtype == torch.int32 and q2k_idx.dim() == 4 and q2k_idx.is_contiguous()
     assert q2k_num.dtype == torch.int32 and q2k_num.is_contiguous()
     ib, ih, nqb, cap = q2k_idx.shape
@@ -755,6 +760,76 @@ def vsa_combine(out_s: torch.Tensor, out_c: torch.Tensor, gate: torch.Tensor | N
                                 ptr(out_c), _i32p(row_block), c_int(block_rows), ptr(out),
                                 o_str if o_str is not None else _bsh_strides(out), c_int(B),
                                 c_int(S), c_int(H), c_int(nblk), ptr(seg_tab), c_int(seg_rows), stream_ptr()))
+    return out
+
+
+# ---------------------------------------------------------------- VSA backward (padded layout: 64-row tiles)
+def vsa_combine_bwd(dO: torch.Tensor, out_c: torch.Tensor, gate: torch.Tensor | None, block_len: torch.Tensor,
+                    d_gate: torch.Tensor | None = None):
+    """Backward of vsa_combine (fvb_vsa_combine_bwd). dO/gate/d_gate: [B, S, H, 128] views, S = 64 * nblk; out_c
+    [B, H, nblk, 128] contiguous; block_len int32 [nblk]. d_gate (output, written when given) = dO * out_c on the valid
+    rows and 0 on the pad rows (pad rows are not tokens: dO there counts as zero).
+    Returns (d_out_c bf16 [B, H, nblk, 128], the same transposed [B, H, 128, nblk] as a view of a [.., ldt] buffer):
+    d_out_c = sum over each tile's valid rows of dO * gate (of dO without a gate), fp32 in a fixed order."""
+    for n, t in (("dO", dO), ("out_c", out_c), ("gate", gate), ("d_gate", d_gate)):
+        if t is not None:
+            _require_cuda_bf16(t, n)
+    B, S, H, d = dO.shape
+    nblk = out_c.shape[2]
+    if d != 128 or S != 64 * nblk or out_c.shape != (B, H, nblk, d) or not out_c.is_contiguous():
+        raise FvbError("dO must be [B, 64 * nblk, H, 128] and out_c contiguous [B, H, nblk, 128]")
+    if d_gate is not None and gate is None:
+        raise FvbError("d_gate needs the gate")
+    _check_i32(block_len, "block_len", nblk)
+    d_out_c = torch.empty((B, H, nblk, d), dtype=torch.bfloat16, device=dO.device)
+    ldt = (nblk + 7) // 8 * 8
+    d_out_c_t = torch.empty((B, H, d, ldt), dtype=torch.bfloat16, device=dO.device)
+    check(lib().fvb_vsa_combine_bwd(ptr(dO), _bsh_strides(dO), ptr(gate), _bsh_strides(gate) if gate is not None else None,
+                                    ptr(out_c), _i32p(block_len), c_int(B), c_int(S), c_int(H), c_int(nblk), ptr(d_gate),
+                                    _bsh_strides(d_gate) if d_gate is not None else None, ptr(d_out_c), ptr(d_out_c_t),
+                                    c_int64(ldt), stream_ptr()))
+    return d_out_c, d_out_c_t[..., :nblk]
+
+
+def softmax_rows_bwd(p: torch.Tensor, dp: torch.Tensor, scale: float = 1.0, want_transposed: bool = False):
+    """Backward of softmax_rows over square blocks (fvb_softmax_rows_bwd). p (the softmax output) and dp: [batch, n, n] bf16
+    views of [batch, n, ld] buffers with the same ld (a multiple of 8), like softmax_rows' and gemm_batched's outputs.
+    Returns ds = bf16(p * (dp - rowsum(dp * p)) * scale) [batch, n, n] (a view of a [.., ld] buffer), and with
+    want_transposed also ds^T and p^T in that layout: the K-major operands of the products that contract over rows."""
+    _require_cuda_bf16(p, "p")
+    _require_cuda_bf16(dp, "dp")
+    batch, n, n2 = p.shape
+    ld = p.stride(1)
+    ok = (n == n2 and dp.shape == p.shape and p.stride(2) == 1 and dp.stride(2) == 1 and dp.stride(1) == ld and ld % 8 == 0
+          and p.stride(0) == n * ld and dp.stride(0) == n * ld)
+    if not ok:
+        raise FvbError("p and dp must be [batch, n, n] views of [batch, n, ld] buffers with one ld (a multiple of 8)")
+    alloc = lambda: torch.empty((batch, n, ld), dtype=torch.bfloat16, device=p.device)
+    ds = alloc()
+    ds_t, p_t = (alloc(), alloc()) if want_transposed else (None, None)
+    check(lib().fvb_softmax_rows_bwd(ptr(p), ptr(dp), c_int64(ld), c_int(batch), c_int(n), c_float(scale), ptr(ds), ptr(ds_t),
+                                     ptr(p_t), stream_ptr()))
+    if want_transposed:
+        return ds[..., :n], ds_t[..., :n], p_t[..., :n]
+    return ds[..., :n]
+
+
+def block_mean_bwd(dx_s: torch.Tensor, d_mean: torch.Tensor, block_len: torch.Tensor, out: torch.Tensor | None = None):
+    """Backward of block_mean in the padded layout added to dx_s (fvb_block_mean_bwd): dx = dx_s + d_mean / len on the valid
+    rows of each 64-row tile, 0 on its pad rows. dx_s / out: [B, S, H, 128] views, S = 64 * nblk (out may be dx_s: in place);
+    d_mean [B, H, nblk, 128] contiguous; block_len int32 [nblk]."""
+    _require_cuda_bf16(dx_s, "dx_s")
+    _require_cuda_bf16(d_mean, "d_mean")
+    B, S, H, d = dx_s.shape
+    nblk = d_mean.shape[2]
+    if d != 128 or S != 64 * nblk or d_mean.shape != (B, H, nblk, d) or not d_mean.is_contiguous():
+        raise FvbError("dx_s must be [B, 64 * nblk, H, 128] and d_mean contiguous [B, H, nblk, 128]")
+    _check_i32(block_len, "block_len", nblk)
+    if out is None:
+        out = torch.empty((B, S, H, d), dtype=torch.bfloat16, device=dx_s.device)
+    _require_cuda_bf16(out, "out")
+    check(lib().fvb_block_mean_bwd(ptr(dx_s), _bsh_strides(dx_s), ptr(d_mean), _i32p(block_len), c_int(B), c_int(H), c_int(S),
+                                   c_int(nblk), ptr(out), _bsh_strides(out), stream_ptr()))
     return out
 
 

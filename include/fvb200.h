@@ -409,6 +409,51 @@ int fvb_gather_rows(const void* in, int64_t in_batch_stride, int64_t in_ld, cons
                     int64_t out_batch_stride, int64_t out_ld, int64_t n_out, int width, int B, void* stream);
 
 /* --------------------------------------------------------------------------------------------
+ * Video Sparse Attention backward, padded layout only: S = 64 * nblk token rows, tile i = rows [64 i, 64 i + 64) of which
+ * the first len[i] = block_len[i] (variable_block_sizes) are valid. The backward of video_sparse_attn
+ * (fastvideo-kernel/python/fastvideo_kernel/ops.py:65-133) as torch autograd differentiates it, top-k selection excluded:
+ *   combine:      fvb_vsa_combine_bwd
+ *   compression:  d_attn = d_out_c v_c^T,  d_v_c = attn^T d_out_c  (fvb_gemm_batched_bf16),
+ *                 d_scores' = fvb_softmax_rows_bwd(attn, d_attn, scale = 1 / sqrt(d)),
+ *                 d_q_c = d_scores' k_c,  d_k_c = d_scores'^T q_c  (fvb_gemm_batched_bf16)
+ *   sparse:       dq_s, dk_s, dv_s = fvb_attention_blocklist_bwd
+ *   block means:  fvb_block_mean_bwd (dq from dq_s and d_q_c, dk and dv likewise)
+ *
+ * Pad rows are not tokens: every gradient below treats dO there as zero (the forward's sparse-branch rows there are zero,
+ *   and its LSE is -inf, so fvb_attention_blocklist_bwd gives them no weight either).
+ *
+ * fvb_vsa_combine_bwd: backward of fvb_vsa_combine. dO, gate, d_gate [B, S, H, 128] through (b, s, h) element strides
+ *   (multiples of 8); out_c, d_out_c bf16 [B, H, nblk, 128] contiguous.
+ *   d_gate[t, c] = bf16(dO[t, c] * out_c[tile(t), c]) on the valid rows, 0 on the pad rows (only when d_gate != NULL)
+ *   d_out_c[i, c] = bf16(sum over the valid rows t of tile i of dO[t, c] * gate[t, c]); gate == NULL: of dO[t, c]
+ *   The products are exact in fp32; the sum is fp32 in a fixed order (16 row-group partial sums, each over its rows in
+ *   order, then the 16 partials in order), so the same inputs give the same bits. d_out_c_t (optional) receives the same
+ *   values transposed, [B, H, 128, ldt] (ldt >= nblk): the K-major operand of d_v_c = attn^T d_out_c.
+ *
+ * fvb_softmax_rows_bwd: backward of fvb_softmax_rows over batch square blocks [n, n] (n <= 8192): p = the softmax output
+ *   and dp = its gradient, bf16, block b at base + b * n * ld, rows of stride ld (a multiple of 8, >= n), 16-byte aligned.
+ *   r[i] = sum_j dp[i, j] * p[i, j]                         (fp32 fused multiply-adds, a fixed order)
+ *   ds[i, j] = bf16((p[i, j] * (dp[i, j] - r[i])) * scale)   (fp32 round-to-nearest, in that order)
+ *   Same layout for ds; ds_t (optional) receives ds transposed (ds_t[j, i] = ds[i, j]) and p_t (optional) p transposed,
+ *   both in the same [batch, n, ld] layout. scale = 1 / sqrt(d) folds the score scaling of q_c k_c^T / sqrt(d) into d_scores.
+ *
+ * fvb_block_mean_bwd: backward of fvb_block_mean (padded layout) added to a gradient that already reaches the rows:
+ *   dx[t, c] = bf16(dx_s[t, c] + d_mean[tile(t), c] / len[tile(t)])   for the valid rows t (fp32 division, then addition)
+ *   dx[t, c] = 0                                                        for the pad rows
+ *   dx_s, dx [B, S, H, 128] through (b, s, h) element strides (multiples of 8); dx may be dx_s (in place). d_mean bf16
+ *   [B, H, nblk, 128] contiguous.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_vsa_combine_bwd(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides,
+                        const void* out_c, const int32_t* block_len, int B, int S, int H, int nblk, void* d_gate,
+                        const int64_t* dg_strides, void* d_out_c, void* d_out_c_t, int64_t ldt, void* stream);
+
+int fvb_softmax_rows_bwd(const void* p, const void* dp, int64_t ld, int batch, int n, float scale, void* ds, void* ds_t,
+                         void* p_t, void* stream);
+
+int fvb_block_mean_bwd(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_len, int B,
+                       int H, int S, int nblk, void* dx, const int64_t* dx_strides, void* stream);
+
+/* --------------------------------------------------------------------------------------------
  * Wan VAE decode (channels-last frames x[t][h][w][c], bf16)
  * -------------------------------------------------------------------------------------------- */
 /* out_f32[M, N] = (A[M, K] @ B[N, K]^T) * scale, fp32 output (attention logits of WanAttentionBlock). */
