@@ -61,6 +61,8 @@ class B200AttentionImpl:
     def forward(self, query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, attn_metadata=None) -> torch.Tensor:
         if attn_metadata is not None and getattr(attn_metadata, "attn_mask", None) is not None:
             raise NotImplementedError("dense boolean masks: use block lists (block_sparse_attn_from_indices / STA)")
+        if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
+            return _DenseAttnFn.apply(query, key, value, self.softmax_scale)
         return ops.attention(query, key, value, softmax_scale=self.softmax_scale)
 
 
@@ -220,6 +222,33 @@ def _lists_to_map(q2k_idx: torch.Tensor, q2k_num: torch.Tensor, nkv: int) -> tor
     bmap = torch.zeros((*q2k_idx.shape[:3], nkv + 1), dtype=torch.bool, device=q2k_idx.device)
     bmap.scatter_(3, torch.where(valid, q2k_idx, nkv).long(), True)
     return bmap[..., :nkv]
+
+
+def _usable_strides(t: torch.Tensor) -> bool:
+    """True when the attention kernels can read t ([B, S, H, 128]) in place: unit channel stride, (b, s, h) strides that are
+    non-zero multiples of 8 (TMA), a 16-byte aligned base."""
+    return t.stride(3) == 1 and all(s != 0 and s % 8 == 0 for s in t.stride()[:3]) and t.data_ptr() % 16 == 0
+
+
+class _DenseAttnFn(torch.autograd.Function):
+    """Dense attention on [B, S, H, 128] views: forward on fvb_attention_fwd (the output is the no-grad call's, bit for bit),
+    backward on fvb_attention_bwd -- what the reference's FlashAttention / SDPA backends give autograd."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, softmax_scale):
+        out, lse = ops.attention(q, k, v, softmax_scale=softmax_scale, return_lse=True)
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.softmax_scale = softmax_scale
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_o):
+        q, k, v, out, lse = ctx.saved_tensors
+        go = grad_o.to(torch.bfloat16)
+        if not _usable_strides(go):
+            go = go.contiguous()
+        dq, dk, dv = ops.attention_bwd(q, k, v, out, lse, go, softmax_scale=ctx.softmax_scale)
+        return dq, dk, dv, None
 
 
 class _BlockSparseAttnFn(torch.autograd.Function):

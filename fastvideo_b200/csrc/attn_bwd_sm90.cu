@@ -270,9 +270,300 @@ __global__ void __launch_bounds__(BW_THREADS) bwd_dkdv_kernel(BwdParams p) {
   }
 }
 
+// ---------------------------------------------------------------- dense backward (fvb_attention_bwd): wgmma + TMA
+// Two kernels, no float atomics:
+//   KV = true : a CTA owns two 64-key tiles (one per consumer warpgroup) and walks every 64-row q tile:
+//               S^T = K Q^T, dP^T = V dO^T (SS, m64n64k16), dV += P^T dO, dK += dS^T Q (RS, m64n128k16, dO / Q as the
+//               transposed B operand, as the forward reads V). lse and delta are per column here: the producer warp stages
+//               them in shared memory with each q tile (+inf / 0 for rows >= Sq, so those columns give P = dS = 0).
+//   KV = false: a CTA owns two 64-row q tiles and walks every 64-key tile: S = Q K^T, dP = dO V^T (SS), dQ += dS K (RS).
+// Warp roles as in the forward: warpgroup 0 is the producer (one TMA warp; setmaxnreg 24), warpgroups 1 and 2 consume
+// (setmaxnreg 240: the KV kernel holds two 64 x 128 fp32 accumulators next to the 64 x 64 S^T and dP^T).
+// Keys >= Skv get P = 0 explicitly (TMA zero fill gives S = 0 there, and exp2(0 - lse) is not 0).
+constexpr int DB_THREADS = 384;
+constexpr int DB_STAGES = 3;
+constexpr int DB_TILE = 64 * 128 * 2;  // 16 KB: [d half (2)][64 rows][128 B], the forward's tile
+constexpr int DB_HALF = 64 * 128;
+constexpr int DB_SMEM = 1024 + 4 * DB_TILE + DB_STAGES * 2 * DB_TILE + DB_STAGES * 2 * 64 * 4 + 256;
+
+struct DenseBwdParams {
+  __nv_bfloat16 *out0, *out1;  // KV: dk, dv; else dq
+  BwdStr so0, so1;
+  const float* lse;
+  int64_t lse_stride_b, lse_stride_h;
+  const float* delta;  // [B, H, Sq]
+  int Sq, Skv, H;
+  float scale, scale_log2;
+};
+
+template <bool KV>
+__global__ void __launch_bounds__(DB_THREADS, 1)
+attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+                      const DenseBwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // resident: [warpgroup (2)][operand (2)][tile] -- KV: (K, V), else (Q, dO); ring: [stage][operand (2)][tile] -- KV:
+  // (Q, dO), else (K, V)
+  uint8_t* sRes = smem;
+  uint8_t* sRing = smem + 4 * DB_TILE;
+  float* sLse = reinterpret_cast<float*>(sRing + DB_STAGES * 2 * DB_TILE);  // [stage][64] (KV only)
+  float* sDelta = sLse + DB_STAGES * 64;
+  uint64_t* res_full = reinterpret_cast<uint64_t*>(sDelta + DB_STAGES * 64);
+  uint64_t* full = res_full + 1;
+  uint64_t* empty = full + DB_STAGES;
+
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int n_walk = KV ? (p.Sq + 63) / 64 : (p.Skv + 63) / 64;
+  const int64_t bh = int64_t(b) * p.H + h;
+  if (threadIdx.x == 0) {
+    mbar_init(res_full, 1);
+    for (int i = 0; i < DB_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);  // lane 0 of each consumer warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  if (wg == 0) {
+    // ------------------------------ producer: warp 0 (all lanes wait; lane 0 issues TMA) ------------------------------
+    reg_dealloc<24>();
+    if (warp != 0) return;
+    const CUtensorMap* res0 = KV ? &tmK : &tmQ;
+    const CUtensorMap* res1 = KV ? &tmV : &tmdO;
+    const CUtensorMap* ring0 = KV ? &tmQ : &tmK;
+    const CUtensorMap* ring1 = KV ? &tmdO : &tmV;
+    if (lane == 0) {
+      tma_prefetch_desc(ring0);
+      tma_prefetch_desc(ring1);
+      mbar_expect_tx(res_full, 4 * DB_TILE);
+      for (int s = 0; s < 2; ++s)
+        for (int hf = 0; hf < 2; ++hf) {
+          const int row0 = (2 * blockIdx.x + s) * 64;
+          tma_load_4d(sRes + (2 * s) * DB_TILE + hf * DB_HALF, res0, res_full, hf * 64, row0, h, b);
+          tma_load_4d(sRes + (2 * s + 1) * DB_TILE + hf * DB_HALF, res1, res_full, hf * 64, row0, h, b);
+        }
+    }
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = 0; t < n_walk; ++t) {
+      mbar_wait(&empty[stage], phase ^ 1);
+      if constexpr (KV) {
+        for (int r = lane; r < 64; r += 32) {
+          const int q = t * 64 + r;
+          sLse[stage * 64 + r] = q < p.Sq ? __ldg(p.lse + int64_t(b) * p.lse_stride_b + int64_t(h) * p.lse_stride_h + q) : INFINITY;
+          sDelta[stage * 64 + r] = q < p.Sq ? __ldg(p.delta + bh * p.Sq + q) : 0.f;
+        }
+        __syncwarp();
+      }
+      if (lane == 0) {
+        uint8_t* dst = sRing + stage * 2 * DB_TILE;
+        mbar_expect_tx(&full[stage], 2 * DB_TILE);  // also the arrive that publishes the staged lse / delta
+        for (int hf = 0; hf < 2; ++hf) {
+          tma_load_4d(dst + hf * DB_HALF, ring0, &full[stage], hf * 64, t * 64, h, b);
+          tma_load_4d(dst + DB_TILE + hf * DB_HALF, ring1, &full[stage], hf * 64, t * 64, h, b);
+        }
+      }
+      if (++stage == DB_STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    return;
+  }
+
+  // ------------------------------ consumers: warpgroup s owns 64 rows (KV: keys, else q rows) ------------------------------
+  reg_alloc<240>();  // 128 x 24 + 256 x 240 = 64 512 of 65 536 registers
+  const int s = wg - 1;
+  const int tq = lane & 3;
+  const int own0 = (2 * blockIdx.x + s) * 64;
+  const int own_rows = max(0, min(64, (KV ? p.Skv : p.Sq) - own0));
+  const uint32_t ra0 = smem_u32(sRes + (2 * s) * DB_TILE), ra1 = smem_u32(sRes + (2 * s + 1) * DB_TILE);
+  // KV: lse / delta come per column from shared memory; else per row, from global once
+  float row_lse[2] = {INFINITY, INFINITY}, row_delta[2] = {0.f, 0.f};
+  if constexpr (!KV) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 16 * warp + (lane >> 2) + 8 * i;
+      if (r < own_rows) {
+        row_lse[i] = __ldg(p.lse + int64_t(b) * p.lse_stride_b + int64_t(h) * p.lse_stride_h + own0 + r);
+        row_delta[i] = __ldg(p.delta + bh * p.Sq + own0 + r);
+      }
+    }
+  }
+  float acc0[64], acc1[64];  // KV: dV, dK; else dQ (acc1 unused)
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
+  mbar_wait(res_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int t = 0; t < n_walk; ++t) {
+    mbar_wait(&full[stage], phase);
+    if (own_rows > 0) {
+      const uint32_t ga0 = smem_u32(sRing + stage * 2 * DB_TILE), ga1 = ga0 + DB_TILE;
+      float sc[32], dp[32];  // KV: S^T, dP^T (rows = keys, columns = q rows); else S, dP
+#pragma unroll
+      for (int i = 0; i < 32; ++i) sc[i] = dp[i] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t off = (k >> 2) * DB_HALF;
+        wgmma_ss<64>(sc, make_desc_kmajor_sw128(ra0 + off) + uint64_t(2 * (k & 3)), make_desc_kmajor_sw128(ga0 + off) + uint64_t(2 * (k & 3)));
+      }
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t off = (k >> 2) * DB_HALF;
+        wgmma_ss<64>(dp, make_desc_kmajor_sw128(ra1 + off) + uint64_t(2 * (k & 3)), make_desc_kmajor_sw128(ga1 + off) + uint64_t(2 * (k & 3)));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sc);
+      wgmma_fence_regs(dp);
+      // P = exp2(S scale log2e - lse), dS = P (dP - delta) scale on rows (16 warp + lane / 4 + 8 i), columns (8 j + 2 tq + c)
+      const int col_valid = KV ? 64 : min(64, p.Skv - t * 64);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float2 cl = make_float2(0.f, 0.f), cd = make_float2(0.f, 0.f);
+        if constexpr (KV) {
+          cl = *reinterpret_cast<const float2*>(sLse + stage * 64 + 8 * j + 2 * tq);
+          cd = *reinterpret_cast<const float2*>(sDelta + stage * 64 + 8 * j + 2 * tq);
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int row = 16 * warp + (lane >> 2) + 8 * i;
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int col = 8 * j + 2 * tq + c;
+            const float l = KV ? (c ? cl.y : cl.x) : row_lse[i];
+            const float dl = KV ? (c ? cd.y : cd.x) : row_delta[i];
+            const bool valid = KV ? row < own_rows : col < col_valid;
+            const int e = 4 * j + 2 * i + c;
+            const float pv = valid ? ex2(fmaf(sc[e], p.scale_log2, -l)) : 0.f;
+            sc[e] = pv;
+            dp[e] = pv * (dp[e] - dl) * p.scale;
+          }
+        }
+      }
+      // P / dS (bf16) as the register A operand, 16 columns per MMA
+      uint32_t pa[4][4], da[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          pa[kk][r] = pack_bf16x2(sc[8 * kk + 2 * r], sc[8 * kk + 2 * r + 1]);
+          da[kk][r] = pack_bf16x2(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
+        }
+      wgmma_fence();
+      if constexpr (KV) {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n128_tb(acc0, pa[kk], make_desc_mnmajor_sw128(ga1 + kk * 16 * 128, DB_HALF));
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n128_tb(acc1, da[kk], make_desc_mnmajor_sw128(ga0 + kk * 16 * 128, DB_HALF));
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n128_tb(acc0, da[kk], make_desc_mnmajor_sw128(ga0 + kk * 16 * 128, DB_HALF));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc0);
+      if constexpr (KV) wgmma_fence_regs(acc1);
+    }
+    if (lane == 0) mbar_arrive(&empty[stage]);
+    if (++stage == DB_STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+
+  // ------------------------------ epilogue: bf16 rows < own_rows ------------------------------
+  auto store = [&](const float(&acc)[64], __nv_bfloat16* base, const BwdStr& st) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 16 * warp + (lane >> 2) + 8 * i;
+      if (r >= own_rows) continue;
+      __nv_bfloat16* op = base + int64_t(b) * st.b + int64_t(own0 + r) * st.s + int64_t(h) * st.h;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<uint32_t*>(op + 8 * j + 2 * tq) = pack_bf16x2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+    }
+  };
+  if constexpr (KV) {
+    store(acc1, p.out0, p.so0);  // dK
+    store(acc0, p.out1, p.so1);  // dV
+  } else {
+    store(acc0, p.out0, p.so0);  // dQ
+  }
+}
+
 }  // namespace fvb
 
 using namespace fvb;
+
+extern "C" int fvb_attention_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
+                                 int64_t lse_stride_b, int64_t lse_stride_h, void* dq, void* dk, void* dv, float* delta_ws,
+                                 const int64_t* q_strides, const int64_t* k_strides, const int64_t* v_strides,
+                                 const int64_t* o_strides, const int64_t* do_strides, const int64_t* dq_strides,
+                                 const int64_t* dk_strides, const int64_t* dv_strides, int B, int H, int Sq, int Skv,
+                                 int head_dim, float softmax_scale, void* stream) {
+  FVB_CHECK_ARG(q && k && v && o && dO && lse && dq && dk && dv && delta_ws, "null pointer");
+  FVB_CHECK_ARG(head_dim == 128, "head_dim must be 128");
+  FVB_CHECK_ARG(B > 0 && H > 0 && Sq > 0 && Skv > 0, "empty problem");
+  FVB_CHECK_ARG(H <= 65535 && B <= 65535, "too many heads / batches");
+  const int64_t* all[8] = {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides};
+  for (auto st : all)
+    for (int i = 0; i < 3; ++i) FVB_CHECK_ARG(st[i] % 8 == 0, "strides must be multiples of 8 elements");
+  auto S3 = [](const int64_t* s) { return BwdStr{s[0], s[1], s[2]}; };
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // delta = rowsum(dO * O), the block-list backward's row kernel
+  BwdParams dp = {};
+  dp.o = reinterpret_cast<const __nv_bfloat16*>(o);
+  dp.dO = reinterpret_cast<const __nv_bfloat16*>(dO);
+  dp.so = S3(o_strides);
+  dp.sdo = S3(do_strides);
+  dp.delta = delta_ws;
+  dp.Sq = Sq;
+  dp.H = H;
+  const int64_t rows = int64_t(B) * H * Sq;
+  bwd_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(dp, B);
+  FVB_CHECK_CUDA(cudaGetLastError());
+
+  CUtensorMap tmQ, tmK, tmV, tmdO;
+  int r;
+  if ((r = make_qkv_tmap(&tmQ, q, Sq, H, B, q_strides[1], q_strides[2], q_strides[0]))) return r;
+  if ((r = make_qkv_tmap(&tmK, k, Skv, H, B, k_strides[1], k_strides[2], k_strides[0]))) return r;
+  if ((r = make_qkv_tmap(&tmV, v, Skv, H, B, v_strides[1], v_strides[2], v_strides[0]))) return r;
+  if ((r = make_qkv_tmap(&tmdO, dO, Sq, H, B, do_strides[1], do_strides[2], do_strides[0]))) return r;
+  DenseBwdParams p = {};
+  p.lse = lse;
+  p.lse_stride_b = lse_stride_b;
+  p.lse_stride_h = lse_stride_h;
+  p.delta = delta_ws;
+  p.Sq = Sq;
+  p.Skv = Skv;
+  p.H = H;
+  p.scale = softmax_scale;
+  p.scale_log2 = softmax_scale * 1.4426950408889634f;
+  static bool configured = false;
+  if (!configured) {
+    FVB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dense_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_SMEM));
+    FVB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dense_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_SMEM));
+    configured = true;
+  }
+  p.out0 = reinterpret_cast<__nv_bfloat16*>(dk);
+  p.out1 = reinterpret_cast<__nv_bfloat16*>(dv);
+  p.so0 = S3(dk_strides);
+  p.so1 = S3(dv_strides);
+  attn_bwd_dense_kernel<true><<<dim3((Skv + 127) / 128, H, B), DB_THREADS, DB_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  p.out0 = reinterpret_cast<__nv_bfloat16*>(dq);
+  p.out1 = nullptr;
+  p.so0 = S3(dq_strides);
+  attn_bwd_dense_kernel<false><<<dim3((Sq + 127) / 128, H, B), DB_THREADS, DB_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
 
 extern "C" int fvb_attention_blocklist_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO,
                                            const float* lse, void* dq, void* dk, void* dv, float* delta_ws,

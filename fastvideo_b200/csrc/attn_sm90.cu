@@ -457,14 +457,6 @@ static int launch_kernel(const CUtensorMap& tmQ, const CUtensorMap& tmK, const C
   return FVB_OK;
 }
 
-static int make_qkv_tmap(CUtensorMap* tm, const void* base, int64_t S, int64_t H, int64_t B, int64_t stride_s,
-                         int64_t stride_h, int64_t stride_b) {
-  uint64_t dims[4] = {(uint64_t)ATT_D, (uint64_t)S, (uint64_t)H, (uint64_t)B};
-  uint64_t str[4] = {2, (uint64_t)stride_s * 2, (uint64_t)stride_h * 2, (uint64_t)stride_b * 2};
-  uint32_t box[4] = {64, 64, 1, 1};
-  return make_tmap_bf16(tm, base, 4, dims, str, box);
-}
-
 static int launch_attention(const void* q, const void* k, const void* v, const int64_t* q_strides, const int64_t* k_strides,
                             const int64_t* v_strides, const int64_t* o_strides, AttnParams& p, int n_pairs, void* stream) {
   for (int i = 0; i < 3; ++i)

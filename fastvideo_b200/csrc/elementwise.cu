@@ -637,6 +637,104 @@ static int rw_stages(int row_bytes) {
   return std::max(1, std::min(RW_MAX_STAGES, RW_SMEM_BUDGET / (RW_WARPS * row_bytes)));
 }
 
+// ------------------------------------------------------------------------------------------
+// RMSNorm backward (fvb_rmsnorm_bwd; arithmetic in include/fvb200.h). Block per row, rows blockIdx.x + k * gridDim.x, the
+// row in registers between the statistics pass and the write. Each thread keeps the fp32 dw partial of its own columns
+// across its CTA's rows; the partials are summed over CTAs in CTA order by rmsnorm_bwd_dw_kernel (no atomics).
+// ------------------------------------------------------------------------------------------
+constexpr int RB_CTAS = 528;  // fixed (not per device), so dw's summation order is the same on every GPU
+
+FVB_DEVICE float2 block_sum2(float2 v, float2* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+    v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();  // protect `red` from the previous use
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float2 t = (lane < EW_THREADS / 32) ? red[lane] : make_float2(0.f, 0.f);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    t.x += __shfl_xor_sync(0xffffffffu, t.x, o);
+    t.y += __shfl_xor_sync(0xffffffffu, t.y, o);
+  }
+  return t;
+}
+
+__global__ void __launch_bounds__(EW_THREADS) rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx,
+                                                                 const __nv_bfloat16* __restrict__ w,
+                                                                 const __nv_bfloat16* __restrict__ dy, int64_t lddy,
+                                                                 __nv_bfloat16* __restrict__ dx, int64_t lddx,
+                                                                 float* __restrict__ dw_part, int M, int D, float eps) {
+  __shared__ float2 red[32];
+  const int nchunks = D >> 3;
+  float acc[EW_MAX_CHUNKS][8];
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+  for (int64_t row = blockIdx.x; row < M; row += gridDim.x) {
+    float xv[EW_MAX_CHUNKS][8], dv[EW_MAX_CHUNKS][8];
+    float2 s = make_float2(0.f, 0.f);  // (sum x^2, sum g x)
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        unpack8(*reinterpret_cast<const uint4*>(x + row * ldx + (ch << 3)), xv[c]);
+        unpack8(*reinterpret_cast<const uint4*>(dy + row * lddy + (ch << 3)), dv[c]);
+        float wv[8];
+        if (w != nullptr) unpack8(__ldg(reinterpret_cast<const uint4*>(w) + ch), wv);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float g = w != nullptr ? bf16_round(__fmul_rn(dv[c][i], wv[i])) : dv[c][i];
+          s.x = __fmaf_rn(xv[c][i], xv[c][i], s.x);
+          s.y = __fmaf_rn(g, xv[c][i], s.y);
+        }
+      }
+    }
+    s = block_sum2(s, red);
+    const float r = rsqrtf(__fdiv_rn(s.x, float(D)) + eps);
+    const float k = __fdiv_rn(__fmul_rn(r, s.y), float(D));  // sum_c (g x^) / D
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        float wv[8], o[8];
+        if (w != nullptr) unpack8(__ldg(reinterpret_cast<const uint4*>(w) + ch), wv);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float g = w != nullptr ? bf16_round(__fmul_rn(dv[c][i], wv[i])) : dv[c][i];
+          const float xh = __fmul_rn(xv[c][i], r);
+          o[i] = __fmul_rn(r, __fsub_rn(g, __fmul_rn(xh, k)));
+          acc[c][i] = __fmaf_rn(dv[c][i], bf16_round(xh), acc[c][i]);
+        }
+        *reinterpret_cast<uint4*>(dx + row * lddx + (ch << 3)) = pack8(o);
+      }
+    }
+  }
+  if (dw_part == nullptr) return;
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+    const int ch = threadIdx.x + c * EW_THREADS;
+    if (ch < nchunks) {
+      float4* dst = reinterpret_cast<float4*>(dw_part + int64_t(blockIdx.x) * D + (ch << 3));
+      dst[0] = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]);
+      dst[1] = make_float4(acc[c][4], acc[c][5], acc[c][6], acc[c][7]);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) rmsnorm_bwd_dw_kernel(const float* __restrict__ dw_part, int nparts, int D,
+                                                              __nv_bfloat16* __restrict__ dw) {
+  const int col = blockIdx.x * 256 + threadIdx.x;
+  if (col >= D) return;
+  float s = 0.f;
+  for (int i = 0; i < nparts; ++i) s = __fadd_rn(s, __ldg(dw_part + int64_t(i) * D + col));
+  dw[col] = __float2bfloat16_rn(s);
+}
+
 }  // namespace fvb
 
 using namespace fvb;
@@ -784,5 +882,31 @@ extern "C" int fvb_rmsnorm_rope(void* x0, const void* w0, int64_t ld0, void* x1,
     else rmsnorm_rope_kernel<false><<<grid, EW_THREADS, 0, st>>>(a, cos_t, sin_t, rope_row, D, head_dim, eps);
   }
   FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_rmsnorm_bwd_workspace_bytes(int M, int D) {
+  return int64_t(std::max(1, std::min(M, RB_CTAS))) * std::max(D, 0) * 4;
+}
+
+extern "C" int fvb_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const void* dy, int64_t lddy, void* dx, int64_t lddx,
+                               void* dw, float* workspace, int64_t workspace_bytes, int M, int D, float eps, void* stream) {
+  FVB_CHECK_ARG(x && dy && dx, "null pointer");
+  FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
+  FVB_CHECK_ARG(ldx % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0, "strides must be multiples of 8");
+  FVB_CHECK_ARG(dw == nullptr || w != nullptr, "dw needs the weight");
+  const int ctas = std::min(M, RB_CTAS);
+  if (dw != nullptr)
+    FVB_CHECK_ARG(workspace != nullptr && workspace_bytes >= fvb_rmsnorm_bwd_workspace_bytes(M, D), "workspace too small");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  rmsnorm_bwd_kernel<<<ctas, EW_THREADS, 0, st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<const __nv_bfloat16*>(w),
+      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, reinterpret_cast<__nv_bfloat16*>(dx), lddx,
+      dw != nullptr ? workspace : nullptr, M, D, eps);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  if (dw != nullptr) {
+    rmsnorm_bwd_dw_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace, ctas, D, reinterpret_cast<__nv_bfloat16*>(dw));
+    FVB_CHECK_CUDA(cudaGetLastError());
+  }
   return FVB_OK;
 }

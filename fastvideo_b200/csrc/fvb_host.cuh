@@ -89,6 +89,16 @@ inline int make_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint
   return make_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, rank, dims, strides_bytes, box, swz);
 }
 
+// Tensor map of one bf16 operand of the head_dim-128 attention kernels: [B][H][S][128] addressed through (b, s, h) element
+// strides, 64-row x 64-channel boxes (one 128B-swizzled half of a 64 x 128 tile).
+inline int make_qkv_tmap(CUtensorMap* tm, const void* base, int64_t S, int64_t H, int64_t B, int64_t stride_s,
+                         int64_t stride_h, int64_t stride_b) {
+  uint64_t dims[4] = {128, (uint64_t)S, (uint64_t)H, (uint64_t)B};
+  uint64_t str[4] = {2, (uint64_t)stride_s * 2, (uint64_t)stride_h * 2, (uint64_t)stride_b * 2};
+  uint32_t box[4] = {64, 64, 1, 1};
+  return make_tmap_bf16(tm, base, 4, dims, str, box);
+}
+
 inline int sm_count() {
   static int n = 0;
   if (n == 0) {

@@ -602,6 +602,51 @@ def attention_blocklist_bwd(q, k, v, o, lse, dO, q2k_idx, q2k_num, k2q_idx, k2q_
     return dq, dk, dv
 
 
+def attention_bwd(q, k, v, o, lse, dO, softmax_scale=None):
+    """fvb_attention_bwd: backward of the dense attention(). q/o/dO: [B, Sq, H, 128], k/v: [B, Skv, H, 128] bf16 views ((b, s, h)
+    strides multiples of 8, as the forward takes them); lse fp32 [B, H, Sq] (unit stride along Sq), as attention(...,
+    return_lse=True) returns it. Returns contiguous (dq, dk, dv) with q's / k's / v's shapes (BSHD)."""
+    for n, t in (("q", q), ("k", k), ("v", v), ("o", o), ("dO", dO)):
+        _require_cuda_bf16(t, n)
+    B, Sq, H, d = q.shape
+    Skv = k.shape[1]
+    if softmax_scale is None:
+        softmax_scale = d ** -0.5
+    if (k.shape != (B, Skv, H, d) or v.shape != k.shape or o.shape != q.shape or dO.shape != q.shape
+            or lse.dtype != torch.float32 or lse.shape != (B, H, Sq) or lse.stride(2) != 1):
+        raise FvbError("attention_bwd: q/o/dO [B, Sq, H, 128], k/v [B, Skv, H, 128], lse fp32 [B, H, Sq]")
+    dq = torch.empty((B, Sq, H, d), dtype=torch.bfloat16, device=q.device)
+    dk = torch.empty((B, Skv, H, d), dtype=torch.bfloat16, device=q.device)
+    dv = torch.empty((B, Skv, H, d), dtype=torch.bfloat16, device=q.device)
+    delta = torch.empty((B * H * Sq,), dtype=torch.float32, device=q.device)
+    check(lib().fvb_attention_bwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(dO), _f32p(lse), c_int64(lse.stride(0)),
+                                  c_int64(lse.stride(1)), ptr(dq), ptr(dk), ptr(dv), _f32p(delta), _bsh_strides(q),
+                                  _bsh_strides(k), _bsh_strides(v), _bsh_strides(o), _bsh_strides(dO), _bsh_strides(dq),
+                                  _bsh_strides(dk), _bsh_strides(dv), c_int(B), c_int(H), c_int(Sq), c_int(Skv), c_int(d),
+                                  c_float(softmax_scale), stream_ptr()))
+    return dq, dk, dv
+
+
+def rmsnorm_bwd(x: torch.Tensor, w: torch.Tensor | None, dy: torch.Tensor, eps: float = 1e-6, want_dw: bool = True):
+    """fvb_rmsnorm_bwd: backward of rmsnorm_rope_(x, w) without RoPE. x, dy: [M, D] bf16 with unit inner stride; w: bf16 [D]
+    or None (ones). Returns (dx bf16 [M, D], dw bf16 [D], or None without w or with want_dw=False)."""
+    _require_cuda_bf16(x, "x")
+    _require_cuda_bf16(dy, "dy")
+    M, D = x.shape
+    if x.stride(1) != 1 or dy.shape != (M, D) or dy.stride(1) != 1:
+        raise FvbError("rmsnorm_bwd: x and dy must be [M, D] with unit inner stride")
+    if w is not None and (w.dtype != torch.bfloat16 or not w.is_contiguous() or w.numel() != D):
+        raise FvbError("rmsnorm_bwd: w must be a contiguous bf16 [D] tensor")
+    dx = torch.empty((M, D), dtype=torch.bfloat16, device=x.device)
+    want_dw = want_dw and w is not None
+    dw = torch.empty(D, dtype=torch.bfloat16, device=x.device) if want_dw else None
+    ws = _workspace(int(lib().fvb_rmsnorm_bwd_workspace_bytes(c_int(M), c_int(D))), x.device) if want_dw else None
+    check(lib().fvb_rmsnorm_bwd(ptr(x), c_int64(x.stride(0)), ptr(w), ptr(dy), c_int64(dy.stride(0)), ptr(dx),
+                                c_int64(dx.stride(0)), ptr(dw), _f32p(ws), c_int64(ws.numel() if ws is not None else 0),
+                                c_int(M), c_int(D), c_float(eps), stream_ptr()))
+    return dx, dw
+
+
 # ---------------------------------------------------------------- index / mask construction
 def vsa_tile_index(seq_shape, tile_size, device="cuda"):
     """Returns dict of device tensors: tile_partition, reverse_partition, non_pad, untile_combined (int64 [S]),

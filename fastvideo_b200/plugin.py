@@ -38,6 +38,10 @@ What install() registers, and the reference interface each piece stands behind:
                       to forward_cuda for the classes that got one.
   whole block         load_wan_block(): a reference WanTransformerBlock(_VSA)'s state_dict() -> wan_dit.WanBlock.
 
+Training: the dense backend (through B200AttentionImpl, backward fvb_attention_bwd) and RMSNorm.forward_cuda (backward
+fvb_rmsnorm_bwd) are differentiable when grad is enabled and an input requires grad; without grad they run the same
+calls as before. The VSA impl above, the 8-bit backend and the linear methods are forward-only.
+
 There is no CPU fallback anywhere: with non-CUDA tensors these classes raise FvbError exactly like the rest of the
 package. uninstall() restores every patched attribute.
 """
@@ -368,15 +372,44 @@ def rms_norm_forward_cuda(self, x: torch.Tensor, residual: torch.Tensor | None =
     D = x.shape[-1]
     if D != self.hidden_size:
         raise ValueError(f"Expected hidden_size to be {self.hidden_size}, but found: {D}")
-    out = x.reshape(-1, D).clone()
     w = self.weight if self.has_weight else None
-    if w is not None and w.dtype == torch.bfloat16:
+    w_bf16 = w is not None and w.dtype == torch.bfloat16
+    if torch.is_grad_enabled() and (x.requires_grad or (w_bf16 and w.requires_grad)):
+        out = _RmsNormFn.apply(x.reshape(-1, D), w if w_bf16 else None, self.variance_epsilon).view(x.shape)
+        return out if w is None or w_bf16 else out * w
+    out = x.reshape(-1, D).clone()
+    if w_bf16:
         ops.rmsnorm_rope_(out, w.contiguous(), head_dim=128, eps=self.variance_epsilon)
         return out.view(x.shape)
     ones = torch.ones(D, dtype=torch.bfloat16, device=x.device)
     ops.rmsnorm_rope_(out, ones, head_dim=128, eps=self.variance_epsilon)
     out = out.view(x.shape)
     return out if w is None else out * w  # fp32 weight: promoted product, as in the reference
+
+
+class _RmsNormFn(torch.autograd.Function):
+    """bf16(bf16(x * rsqrt(mean(x^2) + eps)) * w) over rows of x [M, D], w bf16 [D] or None (ones): forward on
+    fvb_rmsnorm_rope (the output of the no-grad call, bit for bit), backward on fvb_rmsnorm_bwd. An fp32 weight stays outside
+    (the caller multiplies, and torch differentiates the product), so w here is only ever bf16."""
+
+    @staticmethod
+    def forward(ctx, x, w, eps):
+        out = x.clone()
+        ops.rmsnorm_rope_(out, w.contiguous() if w is not None else torch.ones(x.shape[1], dtype=torch.bfloat16, device=x.device),
+                          head_dim=128, eps=eps)
+        ctx.save_for_backward(x, w)
+        ctx.eps = eps
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        dy = dy.to(torch.bfloat16)
+        if dy.stride(1) != 1 or dy.stride(0) % 8 != 0:
+            dy = dy.contiguous()
+        xc = x if x.stride(1) == 1 and x.stride(0) % 8 == 0 else x.contiguous()
+        dx, dw = ops.rmsnorm_bwd(xc, w.contiguous() if w is not None else None, dy, ctx.eps, want_dw=ctx.needs_input_grad[1])
+        return dx, dw, None
 
 
 def _dispatch_forward(self):

@@ -217,6 +217,19 @@ int fvb_rmsnorm_rope_scatter(const void* x0, const void* w0, int64_t ld0, const 
                              void* y1, int64_t ldy, const int64_t* out_col_offsets, const void* cos_t, const void* sin_t,
                              int rope_f64, const int32_t* rope_row, int M, int D, int head_dim, float eps, void* stream);
 
+/* Backward of fvb_rmsnorm_rope without RoPE, n = bf16(bf16(x * r) * w), for one tensor: x, dy, dx bf16 [M, D] rows (row
+ * strides ldx / lddy / lddx, multiples of 8), w bf16 [D] or NULL (all ones), D a multiple of 8, <= 8192. Per row, fp32:
+ *   r = rsqrt(sum_c x^2 / D + eps) (recomputed from x; the forward stores nothing extra), x^ = x * r,
+ *   g = bf16(dy * w) (g = dy without w), s = sum_c g * x (fp32, the row reduced across the CTA),
+ *   dx = bf16(r * (g - x^ * ((r * s) / D)))          -- (r * s) is sum_c g * x^
+ *   dw[c] = bf16(sum_m float(dy[m, c]) * float(bf16(x^[m, c])))   (dw != NULL, needs w)
+ * dw's sum is deterministic: each of min(M, 528) CTAs sums its rows (rows cta, cta + 528, ...) in row order into an fp32
+ * partial per column, then the partials are added in CTA order and rounded once. No atomics. workspace: device memory of
+ * fvb_rmsnorm_bwd_workspace_bytes(M, D) bytes (only used with dw), 16-byte aligned. */
+int64_t fvb_rmsnorm_bwd_workspace_bytes(int M, int D);
+int fvb_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const void* dy, int64_t lddy, void* dx, int64_t lddx, void* dw,
+                    float* workspace, int64_t workspace_bytes, int M, int D, float eps, void* stream);
+
 /* --------------------------------------------------------------------------------------------
  * Attention forward, head_dim 128, bf16, fp32 softmax. Dense or block-list (VSA / STA) keys.
  * Replaces: SDPAImpl.forward (fastvideo/attention/backends/sdpa.py:122-147), LocalAttention cross-attention
@@ -324,6 +337,24 @@ int fvb_attention_blocklist_bwd(const void* q, const void* k, const void* v, con
                                 const int32_t* q2k_idx, const int32_t* q2k_num, int capq, const int32_t* k2q_idx,
                                 const int32_t* k2q_num, int capk, int64_t idx_stride_b, int64_t idx_stride_h,
                                 int64_t kidx_stride_b, int64_t kidx_stride_h, const int32_t* kv_len, void* stream);
+
+/* Backward of fvb_attention_fwd in dense mode (sched == NULL): dq, dk, dv for any Sq >= 1, Skv >= 1. q, k, v, o, dO, dq,
+ * dk, dv are addressed as in the forward (b, s, h element strides, multiples of 8; base addresses 16-byte aligned), lse is
+ * the forward's (log2 domain, lse[b * lse_stride_b + h * lse_stride_h + s]). delta_ws: fp32 [B * H * Sq] workspace.
+ * Per (b, h), over every key j < Skv, fp32 accumulation:
+ *   delta_i = sum_c dO[i, c] * O[i, c]
+ *   P_ij = exp2(q_i . k_j * softmax_scale * log2 e - lse_i)   (ex2.approx)
+ *   dP_ij = dO_i . v_j         dS_ij = P_ij * (dP_ij - delta_i) * softmax_scale
+ *   dV_j = sum_i bf16(P_ij) dO_i      dK_j = sum_i bf16(dS_ij) q_i      dQ_i = sum_j bf16(dS_ij) k_j
+ * The arithmetic of fvb_attention_blocklist_bwd with every key selected. Deterministic: one kernel owns 128 keys per CTA
+ * and walks every q tile (dK, dV), a second owns 128 q rows and walks every key tile (dQ; it recomputes S and dP); no
+ * float atomics. Rows past Sq (keys past Skv) are neither read into the sums nor stored. wgmma + TMA (csrc/attn_bwd_sm90.cu). */
+int fvb_attention_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
+                      int64_t lse_stride_b, int64_t lse_stride_h, void* dq, void* dk, void* dv, float* delta_ws,
+                      const int64_t* q_strides, const int64_t* k_strides, const int64_t* v_strides, const int64_t* o_strides,
+                      const int64_t* do_strides, const int64_t* dq_strides, const int64_t* dk_strides,
+                      const int64_t* dv_strides, int B, int H, int Sq, int Skv, int head_dim, float softmax_scale,
+                      void* stream);
 
 /* --------------------------------------------------------------------------------------------
  * Index / mask construction (integer, bit-exact with the reference)
