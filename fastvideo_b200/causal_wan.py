@@ -30,8 +30,9 @@ from dataclasses import dataclass
 import torch
 
 from . import ops
+from .distributed import out_proj_sp
 from .rope import get_rotary_pos_embed
-from .wan_dit import WanBlock, WanDiT, WanDiTConfig
+from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail
 
 GLOBAL_ATTN_COMPAT_MAX_LATENT_FRAMES = 21  # causal_wanvideo.py:32
 
@@ -193,13 +194,6 @@ def _roped_window(cache: "KVCache", k0: int, k1: int, cos: torch.Tensor, sin: to
     return kr[:k1 - k0].view(k1 - k0, Hc, d)
 
 
-class CrossAttnCache:
-    """crossattn_cache entry (wanvideo.py:202-211): text K/V computed on the first call of a rollout."""
-
-    def __init__(self):
-        self.kv = None
-
-
 def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb: torch.Tensor, cos: torch.Tensor,
                          sin: torch.Tensor, cache: KVCache, xcache: CrossAttnCache | None, current_start: int,
                          cfg: WanDiTConfig, ccfg: CausalConfig, frame_seqlen: int | None = None) -> torch.Tensor:
@@ -209,19 +203,13 @@ def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb
     if ccfg.rope_cache_policy not in ("absolute", "relativistic"):
         raise ops.FvbError(f"unknown rope_cache_policy {ccfg.rope_cache_policy!r}")
     rel = ccfg.rope_cache_policy == "relativistic"
-    if temb.dtype != torch.bfloat16 or blk.scale_shift_table.dtype != torch.bfloat16:
-        raise ops.FvbError("the causal block implements the bf16 modulation flow (bf16 temb and scale_shift_table)")
     S, D = x.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
-    nf = temb.shape[0]
-    tpf = S // nf
+    tpf = S // temb.shape[0]
     fs = tpf if frame_seqlen is None else int(frame_seqlen)
-    # e = scale_shift_table + temb in bf16 (causal_wanvideo.py:288); the kernels take fp32 copies of those bf16 values
-    e = (blk.scale_shift_table + temb.unsqueeze(0)).reshape(nf, 6, D).float()
-    shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate = (e[:, i] for i in range(6))  # [F, D] views, stride 6D
-
-    # 1. self-attention over the cached window (causal_wanvideo.py:293-319, 73-185)
-    n1 = ops.layernorm_modulate(x, scale_msa, shift_msa, round_ln=True, eps=cfg.eps, mod_rows=tpf, mod_bf16=True)
+    mod = Modulation.per_frame(blk, temb, tpf)
+    # self-attention over the cached window (causal_wanvideo.py:293-319, 73-185)
+    n1 = mod.norm1(x, cfg.eps)
     q = _scratch(("q", S, D), (S, D), x.device)
     segs, (k0, k1) = cache.advance(current_start, S, ccfg.local_attn_size, fs)
     kf, vf = cache.k.view(cache.size, D), cache.v.view(cache.size, D)
@@ -241,28 +229,8 @@ def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb
         row += n
     kw = _roped_window(cache, k0, k1, cos, sin, d) if rel else cache.k[k0:k1]
     a = ops.attention(q.view(1, S, H, d), kw.unsqueeze(0), cache.v[k0:k1].unsqueeze(0), softmax_scale=d ** -0.5)
-    # to_out + per-frame gated residual (bf16 product), then LayerNorm(affine) of the bf16 residual (layernorm.py:159-213)
-    x = ops.linear_any(a.reshape(S, D), blk.w_o, blk.b_o, ops.EPI_RESID_GATE_BF16R, resid=x, gate=gate_msa, gate_rows=tpf)
-    n2 = ops.layernorm_modulate(x, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps)
-
-    # 2. cross-attention, text K/V cached across the rollout (wanvideo.py:188-222)
-    q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
-    ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
-    if xcache is not None and xcache.kv is not None:
-        kv2 = xcache.kv
-    else:
-        kv2 = ops.linear_any(ctx, blk.w_kv2, blk.b_kv2)
-        ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
-        if xcache is not None:
-            xcache.kv = kv2
-    a2 = ops.attention(q2.unflatten(1, (H, d)).unsqueeze(0), kv2[:, :D].unflatten(1, (H, d)).unsqueeze(0),
-                       kv2[:, D:].unflatten(1, (H, d)).unsqueeze(0), softmax_scale=d ** -0.5).reshape(S, D)
-    x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
-    n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps, mod_rows=tpf, mod_bf16=True)
-
-    # 3. feed-forward + per-frame gated residual (causal_wanvideo.py:338-340)
-    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-    return ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=tpf)
+    y = ops.linear_any(a.reshape(S, D), blk.w_o, blk.b_o, mod.attn_epilogue, resid=x, gate=mod.gate_msa, gate_rows=mod.rows)
+    return block_tail(y, blk, ctx, mod, cfg, xcache)
 
 
 def _require_bf16_model(cfg: WanDiTConfig) -> None:
@@ -272,12 +240,21 @@ def _require_bf16_model(cfg: WanDiTConfig) -> None:
         raise ops.FvbError("the causal rollout runs bf16 attention only: build the model with attention_8bit=False")
 
 
+def _pad_text(text: torch.Tensor, text_len: int) -> torch.Tensor:
+    """text padded with zero rows to text_len before the embedder (causal_wanvideo.py:604-609)."""
+    if text.shape[1] < text_len:
+        text = torch.cat([text, text.new_zeros(1, text_len - text.shape[1], text.shape[2])], 1)
+    return text
+
+
 class CausalWanDiT(WanDiT):
     """CausalWanTransformer3DModel._forward_inference on libfvb200 (batch 1 per call, like the rollout stage)."""
 
     def __init__(self, cfg: WanDiTConfig, state_dict: dict, ccfg: CausalConfig, blocks: list | None = None):
         _require_bf16_model(cfg)
         super().__init__(cfg, state_dict, blocks)
+        if any(blk.w_kv_img is not None for blk in self.blocks):
+            raise ops.FvbError("the causal rollout's cross-attention is text-only: it cannot load image-to-video blocks")
         self.ccfg = ccfg
         self._rope: dict = {}
 
@@ -334,9 +311,7 @@ class CausalWanDiT(WanDiT):
         fs = Hh * Ww
         lay = self.layout((F_, Hh, Ww), latents.device, None)
         cos, sin = self.block_rope_tables(F_, (Hh, Ww), start_frame, latents.device)
-        # text padded with zero rows to text_len before the embedder (causal_wanvideo.py:604-609)
-        if text.shape[1] < cfg.text_len:
-            text = torch.cat([text, text.new_zeros(1, cfg.text_len - text.shape[1], text.shape[2])], 1)
+        text = _pad_text(text, cfg.text_len)
         temb, tproj, ctx = self.condition(timestep.flatten(), text)  # [F, D], [F, 6, D], [1, L, D]
         x = self.patchify(latents.to(torch.bfloat16), lay)[0]
         for i, blk in enumerate(self.blocks):
@@ -428,14 +403,12 @@ class SPCausalWanDiT:
         return kv, [CrossAttnCache() for _ in m.blocks]
 
     def _block(self, x, blk, ctx, temb, cos, sin, cache: KVCache, xcache, current_start):
-        m, st, P, Hl = self.m, self._st, self.world, self.Hl
+        m, st, Hl = self.m, self._st, self.Hl
         cfg, ccfg = m.cfg, m.ccfg
-        D, H, d = cfg.hidden_size, cfg.num_attention_heads, cfg.head_dim
+        D, d = cfg.hidden_size, cfg.head_dim
         fs, S, n = st["fs"], st["S"], st["n"]
-        S_loc, nf = x.shape[0], temb.shape[0]
-        e = (blk.scale_shift_table + temb.unsqueeze(0)).reshape(nf, 6, D).float()
-        shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate = (e[:, i] for i in range(6))
-        n1 = ops.layernorm_modulate(x, scale_msa, shift_msa, round_ln=True, eps=cfg.eps, mod_rows=n, mod_bf16=True)
+        mod = Modulation.per_frame(blk, temb, n)
+        n1 = mod.norm1(x, cfg.eps)
         segs, (k0, k1) = cache.advance(current_start, S, ccfg.local_attn_size, fs)
         # physical cache row of each frame of the block (write segments split at frame boundaries at most)
         frame_row = []
@@ -446,7 +419,7 @@ class SPCausalWanDiT:
         q_base, k_base, v_base = st["q"].data_ptr(), cache.k.data_ptr(), cache.v.data_ptr()
         v_off = st["head_off"] + (v_base - slab.data_ptr()) // 2
         rel = ccfg.rope_cache_policy == "relativistic"
-        for f in range(nf):
+        for f in range(temb.shape[0]):
             rows = slice(f * n, (f + 1) * n)
             drow = frame_row[f] + self.rank * n     # destination row inside the owner's cache
             qrow = f * fs + self.rank * n           # destination row inside the owner's q buffer (block order)
@@ -465,26 +438,7 @@ class SPCausalWanDiT:
         o = ops.attention(st["q"].unsqueeze(0), kw.unsqueeze(0), cache.v[k0:k1].unsqueeze(0), softmax_scale=d ** -0.5)
         ops.scatter_rows_to_segments(o[0].view(S, rowb), st["seg"], n)
         st["hdl"].barrier(channel=1)  # my tokens' heads have arrived from every rank (and everyone is done reading q)
-        y = torch.empty((S_loc, D), dtype=torch.bfloat16, device=x.device)
-        ops.linear_sp(st["back"], S_loc, D, rowb, blk.w_o, blk.b_o, y, D, ops.EPI_RESID_GATE_BF16R, x_seg_len=rowb,
-                      x_seg_stride=S_loc * rowb, resid=x, gate=gate_msa, gate_rows=n)
-        x = y
-        n2 = ops.layernorm_modulate(x, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps)
-        q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
-        ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
-        if xcache is not None and xcache.kv is not None:
-            kv2 = xcache.kv
-        else:
-            kv2 = ops.linear_any(ctx, blk.w_kv2, blk.b_kv2)
-            ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
-            if xcache is not None:
-                xcache.kv = kv2
-        a2 = ops.attention(q2.unflatten(1, (H, d)).unsqueeze(0), kv2[:, :D].unflatten(1, (H, d)).unsqueeze(0),
-                           kv2[:, D:].unflatten(1, (H, d)).unsqueeze(0), softmax_scale=d ** -0.5).reshape(S_loc, D)
-        x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
-        n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps, mod_rows=n, mod_bf16=True)
-        f_ = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-        return ops.linear_any(f_, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16R, resid=x, gate=c_gate, gate_rows=n)
+        return block_tail(out_proj_sp(st["back"], blk, x, mod), blk, ctx, mod, cfg, xcache)
 
     @torch.no_grad()
     def forward_inference(self, latents, text, timestep, kv_cache, crossattn_cache, current_start: int = 0, start_frame: int = 0):
@@ -499,15 +453,12 @@ class SPCausalWanDiT:
         assert fs == st["fs"] and F_ * fs == st["S"]
         lay = m.layout((F_, Hh, Ww), latents.device, None)
         cos, sin = m.block_rope_tables(F_, (Hh, Ww), start_frame, latents.device)
-        if text.shape[1] < cfg.text_len:
-            text = torch.cat([text, text.new_zeros(1, cfg.text_len - text.shape[1], text.shape[2])], 1)
+        text = _pad_text(text, cfg.text_len)
         temb, tproj, ctx = m.condition(timestep.flatten(), text)
         # my rows of the block: for every frame, tokens [rank * n, (rank + 1) * n)
         idx = (torch.arange(F_, device=latents.device)[:, None] * fs + self.rank * n +
                torch.arange(n, device=latents.device)[None, :]).reshape(-1)
-        B, C, T, Hl_, Wl_ = latents.shape
-        patches = latents.to(torch.bfloat16).view(B, C, T // pt, pt, Hl_ // ph, ph, Wl_ // pw, pw) \
-            .permute(0, 2, 4, 6, 1, 3, 5, 7).reshape(F_ * fs, C * pt * ph * pw)
+        patches = m.patches(latents.to(torch.bfloat16))[0]
         x = ops.linear(patches[idx].contiguous(), m.w_patch, m.b_patch)
         qlo = 0
         if m.ccfg.rope_cache_policy == "relativistic":

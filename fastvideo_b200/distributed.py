@@ -149,6 +149,18 @@ def init_from_env(backend: str | None = None):
 # ----------------------------------------------------------------------------------------------------------------
 # sequence-parallel block / model forward (CUDA)
 # ----------------------------------------------------------------------------------------------------------------
+def out_proj_sp(back: torch.Tensor, blk, x: torch.Tensor, mod) -> torch.Tensor:
+    """Self-attention out-projection + gated residual (epilogue and output dtype per the wan_dit.Modulation `mod`) of my
+    S_loc tokens: the return buffer back [P(src), S_loc, Hl, d] is read in place as an A operand K-segmented by source rank."""
+    from . import ops
+    S_loc, D = x.shape
+    seg = back.shape[2] * back.shape[3]
+    y = torch.empty((S_loc, D), dtype=torch.bfloat16 if mod.bf16 else torch.float32, device=x.device)
+    ops.linear_sp(back, S_loc, D, seg, blk.w_o, blk.b_o, y, D, mod.attn_epilogue, x_seg_len=seg, x_seg_stride=S_loc * seg,
+                  resid=x, gate=mod.gate_msa, gate_rows=mod.rows)
+    return y
+
+
 class SPWanDiT:
     """WanDiT sharded over `world` ranks. Every rank holds all weights (replicated, as in the reference)."""
 
@@ -232,37 +244,36 @@ class SPWanDiT:
 
     def block_forward(self, x, blk, ctx, temb6, lay, plan_t, rope_row_local):
         from . import ops, vsa
+        from .wan_dit import Modulation, block_tail
         plan, qkv_off, head_off = plan_t
         cfg = self.m.cfg
-        D, H, d, Hl, P = cfg.hidden_size, cfg.num_attention_heads, cfg.head_dim, plan.local_heads, self.world
+        D, d, Hl, P = cfg.hidden_size, cfg.head_dim, plan.local_heads, self.world
         S_loc, S, S_pad, n_proj = plan.local_seq, plan.seq_len, plan.padded_seq, plan.n_proj
-        e = blk.scale_shift_table + temb6.float()
-        shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate = [t.reshape(D).contiguous() for t in e.chunk(6, dim=1)]
-
-        n1 = ops.layernorm_modulate(x, scale_msa, shift_msa, eps=cfg.eps)
+        mod = Modulation.fp32(blk, temb6)
+        n1 = mod.norm1(x, cfg.eps)
         if self.comm == "push" and P > 1 and self._push_ok(plan, x.device):
             back = self._attention_push(n1, blk, lay, plan, rope_row_local)
-            return self._block_tail(x, blk, ctx, plan, back, gate_msa, c_shift, c_scale, c_gate)
-        send = torch.empty((P, S_loc, n_proj, Hl, d), dtype=torch.bfloat16, device=x.device)
-        ops.linear_sp(n1, S_loc, D, n1.stride(0), blk.w_qkv, blk.b_qkv, send, plan.send_row_stride, out_col_offsets=qkv_off)
-        flat = send.view(-1)
-        qb = flat.as_strided((S_loc, 1), (plan.send_row_stride, 1))
-        kb = flat[Hl * d:].as_strided((S_loc, 1), (plan.send_row_stride, 1))
-        ops.rmsnorm_rope_(qb, blk.norm_q, kb, blk.norm_k, lay.cos, lay.sin, rope_row_local, head_dim=d, eps=cfg.eps,
-                          col_offsets=head_off, shape=(S_loc, D))
-        recv = all_to_all_tokens_to_heads(send, self.group)  # [S_pad, n_proj, Hl, d]
-        q = recv[:S, 0].unsqueeze(0)
-        k = recv[:S, 1].unsqueeze(0)
-        v = recv[:S, 2].unsqueeze(0)
-        o = torch.zeros((1, S_pad, Hl, d), dtype=torch.bfloat16, device=x.device) if S_pad != S else \
-            torch.empty((1, S_pad, Hl, d), dtype=torch.bfloat16, device=x.device)
-        if cfg.vsa:
-            vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=recv[:S, 3].unsqueeze(0), block_off=lay.block_off,
-                                       row_block=lay.row_block, out=o[:, :S])
         else:
-            ops.attention(q, k, v, softmax_scale=d ** -0.5, out=o[:, :S])
-        back = all_to_all_heads_to_tokens(o[0], P, self.group)  # [P(src), S_loc, Hl, d]
-        return self._block_tail(x, blk, ctx, plan, back, gate_msa, c_shift, c_scale, c_gate)
+            send = torch.empty((P, S_loc, n_proj, Hl, d), dtype=torch.bfloat16, device=x.device)
+            ops.linear_sp(n1, S_loc, D, n1.stride(0), blk.w_qkv, blk.b_qkv, send, plan.send_row_stride, out_col_offsets=qkv_off)
+            flat = send.view(-1)
+            qb = flat.as_strided((S_loc, 1), (plan.send_row_stride, 1))
+            kb = flat[Hl * d:].as_strided((S_loc, 1), (plan.send_row_stride, 1))
+            ops.rmsnorm_rope_(qb, blk.norm_q, kb, blk.norm_k, lay.cos, lay.sin, rope_row_local, head_dim=d, eps=cfg.eps,
+                              col_offsets=head_off, shape=(S_loc, D))
+            recv = all_to_all_tokens_to_heads(send, self.group)  # [S_pad, n_proj, Hl, d]
+            q = recv[:S, 0].unsqueeze(0)
+            k = recv[:S, 1].unsqueeze(0)
+            v = recv[:S, 2].unsqueeze(0)
+            o = torch.zeros((1, S_pad, Hl, d), dtype=torch.bfloat16, device=x.device) if S_pad != S else \
+                torch.empty((1, S_pad, Hl, d), dtype=torch.bfloat16, device=x.device)
+            if cfg.vsa:
+                vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=recv[:S, 3].unsqueeze(0), block_off=lay.block_off,
+                                           row_block=lay.row_block, out=o[:, :S])
+            else:
+                ops.attention(q, k, v, softmax_scale=d ** -0.5, out=o[:, :S])
+            back = all_to_all_heads_to_tokens(o[0], P, self.group)  # [P(src), S_loc, Hl, d]
+        return block_tail(out_proj_sp(back, blk, x, mod), blk, ctx, mod, cfg)
 
     def _attention_push(self, n1, blk, lay, plan, rope_row_local):
         """Self-attention with the exchange done by peer-memory stores. Returns the return buffer [P, S_loc, Hl, d]."""
@@ -294,24 +305,6 @@ class SPWanDiT:
         st["h_back"].barrier(channel=1)
         return st["back"]
 
-    def _block_tail(self, x, blk, ctx, plan, back, gate_msa, c_shift, c_scale, c_gate):
-        """Everything after the return exchange: out-projection (A operand K-segmented by source rank), cross-attention, FFN."""
-        from . import ops
-        cfg = self.m.cfg
-        D, H, d, Hl, P = cfg.hidden_size, cfg.num_attention_heads, cfg.head_dim, plan.local_heads, self.world
-        S_loc = plan.local_seq
-        r32 = torch.empty((S_loc, D), dtype=torch.float32, device=x.device)
-        ops.linear_sp(back, S_loc, D, Hl * d, blk.w_o, blk.b_o, r32, D, ops.EPI_RESID_GATE_F32, x_seg_len=Hl * d,
-                      x_seg_stride=S_loc * Hl * d, resid=x, gate=gate_msa)
-        n2, x = ops.layernorm_modulate(r32, None, None, blk.norm2_w, blk.norm2_b, eps=cfg.eps, want_hidden=True)
-
-        from .wan_dit import cross_attention
-        a2 = cross_attention(n2, blk, ctx, cfg)
-        x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
-        n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps)
-        f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-        return ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
-
     @torch.no_grad()
     def forward(self, latents, text, timestep, vsa_sparsity=None):
         from . import ops
@@ -325,9 +318,7 @@ class SPWanDiT:
         plan = plan_t[0]
         temb, tproj, ctx = m.condition(timestep, text)
         # patchify only this rank's tokens (sequence_model_parallel_shard, wanvideo.py:693)
-        B, C, T, Hh, Ww = latents.shape
-        patches = latents.to(torch.bfloat16).view(B, C, T // pt, pt, Hh // ph, ph, Ww // pw, pw) \
-            .permute(0, 2, 4, 6, 1, 3, 5, 7).reshape(S, C * pt * ph * pw)
+        patches = m.patches(latents.to(torch.bfloat16))[0]
         lo, hi = plan.token_range
         order = lay.perm[lo:hi] if lay.perm is not None else torch.arange(lo, hi, device=latents.device)
         xl = torch.zeros((plan.local_seq, patches.shape[1]), dtype=torch.bfloat16, device=latents.device)

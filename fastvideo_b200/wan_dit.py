@@ -202,12 +202,60 @@ def make_layout(seq_shape, cfg: WanDiTConfig, device, vsa_sparsity: float | None
     return lay
 
 
+@dataclass
+class Modulation:
+    """AdaLN modulation of one block and the rounding flow it implies: fp32 (WanTransformerBlock, wanvideo.py:388-390; one
+    row for all tokens) or bf16 (CausalWanTransformerBlock, causal_wanvideo.py:288; one row per latent frame of `rows`
+    tokens, every modulation / gate product rounded to bf16)."""
+    shift_msa: torch.Tensor
+    scale_msa: torch.Tensor
+    gate_msa: torch.Tensor
+    c_shift: torch.Tensor
+    c_scale: torch.Tensor
+    c_gate: torch.Tensor
+    rows: int = 0  # tokens per modulation row; 0: one row for all tokens
+    bf16: bool = False
+
+    @classmethod
+    def fp32(cls, blk: WanBlock, temb6: torch.Tensor) -> "Modulation":  # temb6: [1, 6, D]
+        e = blk.scale_shift_table + temb6.float()
+        return cls(*[t.reshape(temb6.shape[-1]).contiguous() for t in e.chunk(6, dim=1)])
+
+    @classmethod
+    def per_frame(cls, blk: WanBlock, temb: torch.Tensor, rows: int) -> "Modulation":  # temb: [F, 6, D] bf16
+        if temb.dtype != torch.bfloat16 or blk.scale_shift_table.dtype != torch.bfloat16:
+            raise ops.FvbError("the causal block implements the bf16 modulation flow (bf16 temb and scale_shift_table)")
+        # the kernels take fp32 copies of the bf16 sums; the [F, D] views keep their 6D row stride
+        e = (blk.scale_shift_table + temb.unsqueeze(0)).reshape(temb.shape).float()
+        return cls(*(e[:, i] for i in range(6)), rows=rows, bf16=True)
+
+    def norm1(self, x: torch.Tensor, eps: float) -> torch.Tensor:
+        return ops.layernorm_modulate(x, self.scale_msa, self.shift_msa, round_ln=self.bf16, eps=eps, mod_rows=self.rows,
+                                      mod_bf16=self.bf16)
+
+    @property
+    def attn_epilogue(self) -> int:  # out-projection + gated residual: fp32 output, or bf16 product and output
+        return ops.EPI_RESID_GATE_BF16R if self.bf16 else ops.EPI_RESID_GATE_F32
+
+    @property
+    def ffn_epilogue(self) -> int:
+        return ops.EPI_RESID_GATE_BF16R if self.bf16 else ops.EPI_RESID_GATE_BF16
+
+
+@dataclass
+class CrossAttnCache:
+    """crossattn_cache entry (wanvideo.py:202-211): text K/V computed on the first call of a rollout."""
+    kv: torch.Tensor | None = None
+
+
 I2V_IMAGE_TOKENS = 257  # wanvideo.py:259-260: the first 257 context rows are the CLIP image tokens
 
 
-def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: WanDiTConfig) -> torch.Tensor:
+def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: WanDiTConfig,
+                    xcache: CrossAttnCache | None = None) -> torch.Tensor:
     """WanT2VCrossAttention.forward (wanvideo.py:188-222), or WanI2VCrossAttention.forward (:225-280) when the block
-    carries add_k_proj / add_v_proj: text attention + image-token attention, summed in bf16. Returns [S, D] (pre to_out)."""
+    carries add_k_proj / add_v_proj: text attention + image-token attention, summed in bf16. Returns [S, D] (pre to_out).
+    With `xcache`, the text K/V are computed on the first call and reused afterwards."""
     S, D = n2.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
     hd = lambda t: t.unflatten(1, (H, d)).unsqueeze(0)
@@ -221,10 +269,30 @@ def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: Wan
         img = ops.attention(hd(q2), hd(kvi[:, :D]), hd(kvi[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
         if ctx.shape[0] == 0:
             return img  # zeros_like(q) + img_x
-    kv2 = ops.linear_any(ctx.contiguous(), blk.w_kv2, blk.b_kv2)  # [L, 2D]
-    ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
+    if xcache is not None and xcache.kv is not None:
+        kv2 = xcache.kv
+    else:
+        kv2 = ops.linear_any(ctx.contiguous(), blk.w_kv2, blk.b_kv2)  # [L, 2D]
+        ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
+        if xcache is not None:
+            xcache.kv = kv2
     a2 = ops.attention(hd(q2), hd(kv2[:, :D]), hd(kv2[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
     return a2 if img is None else a2 + img  # `x = x + img_x` on bf16 tensors
+
+
+def block_tail(y: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulation, cfg: WanDiTConfig,
+               xcache: CrossAttnCache | None = None) -> torch.Tensor:
+    """The block after the self-attention out-projection y (fp32 or bf16, per mod.attn_epilogue): LayerNorm(affine),
+    cross-attention, feed-forward (wanvideo.py:415-432, causal_wanvideo.py:321-340). Returns [S, D] bf16."""
+    if mod.bf16:  # LayerNorm of the bf16 residual (layernorm.py:159-213)
+        n2, x = ops.layernorm_modulate(y, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps), y
+    else:  # LayerNorm of the fp32 residual, which also becomes the bf16 residual stream
+        n2, x = ops.layernorm_modulate(y, None, None, blk.norm2_w, blk.norm2_b, eps=cfg.eps, want_hidden=True)
+    a2 = cross_attention(n2, blk, ctx, cfg, xcache)
+    x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
+    n3 = ops.layernorm_modulate(x, mod.c_scale, mod.c_shift, round_ln=True, eps=cfg.eps, mod_rows=mod.rows, mod_bf16=mod.bf16)
+    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+    return ops.linear_any(f, blk.w_2, blk.b_2, mod.ffn_epilogue, resid=x, gate=mod.c_gate, gate_rows=mod.rows)
 
 
 def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torch.Tensor, lay: TokenLayout,
@@ -232,12 +300,9 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
     """x: [S, D] bf16 (one sample), ctx: [L, D] bf16 text states, temb6: [1, 6, D] (timestep_proj). Returns [S, D]."""
     S, D = x.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
-    # wanvideo.py:388-390 -- fp32 modulation
-    e = blk.scale_shift_table + temb6.float()
-    shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate = [t.reshape(D).contiguous() for t in e.chunk(6, dim=1)]
-
-    # 1. self-attention (wanvideo.py:393-415)
-    n1 = ops.layernorm_modulate(x, scale_msa, shift_msa, eps=cfg.eps)
+    mod = Modulation.fp32(blk, temb6)
+    # self-attention (wanvideo.py:393-415)
+    n1 = mod.norm1(x, cfg.eps)
     qkv = ops.linear_any(n1, blk.w_qkv, blk.b_qkv)  # [S, 3D or 4D]
     ops.rmsnorm_rope_(qkv[:, :D], blk.norm_q, qkv[:, D:2 * D], blk.norm_k, lay.cos, lay.sin, lay.rope_row, head_dim=d,
                       eps=cfg.eps)
@@ -252,20 +317,8 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
         a = ops.attention_8bit(ops.quantize_attention_8bit(q, k, v), d ** -0.5)
     else:
         a = ops.attention(q, k, v, softmax_scale=d ** -0.5)
-    a = a.reshape(S, D)
-    # to_out + gated residual in fp32, then LN(affine) and the bf16 residual stream (wanvideo.py:415-421)
-    r32 = ops.linear_any(a, blk.w_o, blk.b_o, ops.EPI_RESID_GATE_F32, resid=x, gate=gate_msa)
-    n2, x = ops.layernorm_modulate(r32, None, None, blk.norm2_w, blk.norm2_b, eps=cfg.eps, want_hidden=True)
-
-    # 2. cross-attention (wanvideo.py:188-222, 424-427)
-    a2 = cross_attention(n2, blk, ctx, cfg)
-    x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
-    n3 = ops.layernorm_modulate(x, c_scale, c_shift, round_ln=True, eps=cfg.eps)
-
-    # 3. feed-forward (wanvideo.py:430-432)
-    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-    x = ops.linear_any(f, blk.w_2, blk.b_2, ops.EPI_RESID_GATE_BF16, resid=x, gate=c_gate)
-    return x
+    y = ops.linear_any(a.reshape(S, D), blk.w_o, blk.b_o, mod.attn_epilogue, resid=x, gate=mod.gate_msa, gate_rows=mod.rows)
+    return block_tail(y, blk, ctx, mod, cfg)
 
 
 class WanDiT:
@@ -331,13 +384,17 @@ class WanDiT:
         ctx = ops.linear(ops.linear(text, self.w_x1, self.b_x1, ops.EPI_BIAS_GELU_TANH), self.w_x2, self.b_x2)
         return temb, tproj.unflatten(1, (6, -1)), ctx
 
-    def patchify(self, latents: torch.Tensor, lay: TokenLayout) -> torch.Tensor:
-        """[B, C, T, H, W] -> [B, S, D]: Conv3d(kernel = stride = patch) as a GEMM over (c, pt, ph, pw) patches
-        (fastvideo/layers/visual_embedding.py:47-55; wanvideo.py:689-690), tokens emitted in layout order."""
+    def patches(self, latents: torch.Tensor) -> torch.Tensor:
+        """[B, C, T, H, W] -> [B, S, C*pt*ph*pw]: the (c, pt, ph, pw) patches of every token, in raster order."""
         B, C, T, Hh, Ww = latents.shape
         pt, ph, pw = self.cfg.patch_size
         x = latents.view(B, C, T // pt, pt, Hh // ph, ph, Ww // pw, pw).permute(0, 2, 4, 6, 1, 3, 5, 7)
-        x = x.reshape(B, -1, C * pt * ph * pw)
+        return x.reshape(B, -1, C * pt * ph * pw)
+
+    def patchify(self, latents: torch.Tensor, lay: TokenLayout) -> torch.Tensor:
+        """[B, C, T, H, W] -> [B, S, D]: Conv3d(kernel = stride = patch) as a GEMM over (c, pt, ph, pw) patches
+        (fastvideo/layers/visual_embedding.py:47-55; wanvideo.py:689-690), tokens emitted in layout order."""
+        x = self.patches(latents)
         if lay.perm is not None:
             x = x[:, lay.perm]
         return ops.linear(x.contiguous(), self.w_patch, self.b_patch)

@@ -116,6 +116,23 @@ def test_oracle_reproduces_reference_relativistic_rollouts(golden_dir):
         assert_equal_or_host_rounding(y, c["y_ref_bf16"], tol=6e-3, name="relativistic model")
 
 
+def test_causal_model_refuses_i2v_blocks():
+    """The causal rollout's cross-attention is text-only (WanT2VCrossAttention): a checkpoint whose blocks carry the I2V
+    image-token projections is refused at load instead of running an image branch the causal reference does not have."""
+    import pytest
+    from fastvideo_b200 import causal_wan, ops, wan_dit
+    cfg = wan_dit.WanDiTConfig(hidden_size=64, num_attention_heads=1, ffn_dim=128, num_layers=1, text_dim=32, freq_dim=16)
+    sd = wan_dit.random_state_dict(cfg, device="cpu")
+    causal_wan.CausalWanDiT(cfg, sd, causal_wan.CausalConfig())  # the text-to-video checkpoint loads
+    D = cfg.hidden_size
+    for n in ("add_k_proj", "add_v_proj"):
+        sd[f"blocks.0.attn2.{n}.weight"] = torch.zeros(D, D, dtype=torch.bfloat16)
+        sd[f"blocks.0.attn2.{n}.bias"] = torch.zeros(D, dtype=torch.bfloat16)
+    sd["blocks.0.attn2.norm_added_k.weight"] = torch.ones(D, dtype=torch.bfloat16)
+    with pytest.raises(ops.FvbError, match="text-only"):
+        causal_wan.CausalWanDiT(cfg, sd, causal_wan.CausalConfig())
+
+
 def test_window_positions_follow_the_reference_order():
     """KVCache.window_positions: the position the relativistic policy gives a physical row equals the row's index in the
     reference's shifted (logical) window, for every ring state of random rollouts."""

@@ -383,7 +383,7 @@ def _free_port():
 
 
 def test_sp_w8_equals_single_rank(tmp_path):
-    """tests/sp_worker_w8.py on 2 ranks: SPWanDiT with int8_weights bit-equal to the single-rank engine (dense and VSA, push
+    """tests/sp_worker.py int8 on 2 ranks: SPWanDiT with int8_weights bit-equal to the single-rank engine (dense and VSA, push
     and NCCL), SPCausalWanDiT with int8_weights within bf16 rounding of it."""
     world = 2
     if torch.cuda.device_count() < world:
@@ -391,7 +391,7 @@ def test_sp_w8_equals_single_rank(tmp_path):
     out = str(tmp_path / f"sp_w8_parity_{world}.json")
     env = dict(os.environ, SP_WORKER_OUT=out)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "sp_worker_w8.py")]
+           "--master-port", str(_free_port()), os.path.join(ROOT, "tests", "sp_worker.py"), "int8"]
     p = subprocess.run(cmd, capture_output=True, text=True, timeout=900, cwd=ROOT, env=env)
     assert p.returncode == 0, (p.stdout[-3000:], p.stderr[-3000:])
     res = json.load(open(out))

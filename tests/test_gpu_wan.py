@@ -111,3 +111,28 @@ def test_sequence_parallel_code_path_world1_matches_single_rank(golden_dir):
     y1 = model.forward(*args)
     y2 = distributed.SPWanDiT(model, 0, 1).forward(*args)
     assert torch.equal(y1, y2)
+
+
+@pytest.mark.parametrize("vsa, weights", [(False, "int8_weights"), (False, "w8a8"), (True, "bf16"), (True, "int8_weights"),
+                                          (True, "w8a8")], ids=lambda v: {False: "dense", True: "vsa"}.get(v, v))
+def test_sequence_parallel_world1_matches_single_rank_vsa_and_int8(golden_dir, vsa, weights):
+    """The world-1 check above with VSA attention and with int8 weights (weight-only and W8A8): the sequence-parallel
+    out-projection and block tail match the single-rank forward bit for bit in every weight format."""
+    from fastvideo_b200 import wan_dit, distributed
+    fmt = {"bf16": {}, "int8_weights": dict(int8_weights=True), "w8a8": dict(int8_weights=True, int8_activations=True)}[weights]
+    g = torch.load(os.path.join(golden_dir, "wan_model_dense.pt"))
+    sd = cuda_sd(g["sd"])
+    cfg = wan_dit.WanDiTConfig(hidden_size=sd["proj_out.weight"].shape[1], num_attention_heads=g["heads"],
+                               ffn_dim=sd["blocks.0.ffn.fc_in.weight"].shape[0], num_layers=2,
+                               text_dim=sd["condition_embedder.text_embedder.fc_in.weight"].shape[1], vsa=vsa, **fmt)
+    if vsa:  # the checkpoint is a dense one: add the VSA gate projections
+        gen = torch.Generator(device="cuda").manual_seed(0)
+        for i in range(2):
+            sd[f"blocks.{i}.to_gate_compress.weight"] = (torch.randn(cfg.hidden_size, cfg.hidden_size, device="cuda", generator=gen) / 16).bfloat16()
+            sd[f"blocks.{i}.to_gate_compress.bias"] = torch.zeros(cfg.hidden_size, device="cuda").bfloat16()
+    model = wan_dit.WanDiT(cfg, sd)
+    args = (g["latents"].cuda(), g["text"].cuda(), g["timestep"].cuda())
+    sparsity = 0.5 if vsa else None
+    y1 = model.forward(*args, vsa_sparsity=sparsity)
+    y2 = distributed.SPWanDiT(model, 0, 1).forward(*args, vsa_sparsity=sparsity)
+    assert torch.equal(y1, y2)
