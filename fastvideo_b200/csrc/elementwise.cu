@@ -735,6 +735,50 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_dw_kernel(const float* __rest
   dw[col] = __float2bfloat16_rn(s);
 }
 
+// ------------------------------------------------------------------------------------------
+// Bias gradient of the bf16 linear (fvb_bias_grad_bf16): db[n] = bf16(sum_m dy[m, n]). blockIdx.y picks 1024 columns
+// (8 per thread), blockIdx.x one of BG_PARTS fixed row sets (rows part, part + BG_PARTS, ...), summed in row order into
+// fp32 partials; rmsnorm_bwd_dw_kernel then adds the partials in part order and rounds once. No atomics: the summation
+// order depends on M and N only.
+// ------------------------------------------------------------------------------------------
+constexpr int BG_PARTS = 256;  // fixed (not per device), so db's summation order is the same on every GPU
+constexpr int BG_THREADS = 128;
+constexpr int BG_UNROLL = 8;  // row loads in flight per thread
+
+__global__ void __launch_bounds__(BG_THREADS) bias_grad_kernel(const __nv_bfloat16* __restrict__ dy, int64_t lddy,
+                                                               float* __restrict__ part, int M, int N, int nparts) {
+  const int col = (blockIdx.y * BG_THREADS + threadIdx.x) * 8;
+  if (col >= N) return;
+  float acc[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  const int64_t step = int64_t(nparts) * lddy;
+  const __nv_bfloat16* p = dy + int64_t(blockIdx.x) * lddy + col;
+  int row = blockIdx.x;
+  for (; row + (BG_UNROLL - 1) * nparts < M; row += BG_UNROLL * nparts) {
+    uint4 v[BG_UNROLL];
+#pragma unroll
+    for (int u = 0; u < BG_UNROLL; ++u) v[u] = __ldg(reinterpret_cast<const uint4*>(p + u * step));
+    p += BG_UNROLL * step;
+#pragma unroll
+    for (int u = 0; u < BG_UNROLL; ++u) {
+      float f[8];
+      unpack8(v[u], f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = __fadd_rn(acc[i], f[i]);
+    }
+  }
+  for (; row < M; row += nparts, p += step) {
+    float f[8];
+    unpack8(__ldg(reinterpret_cast<const uint4*>(p)), f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] = __fadd_rn(acc[i], f[i]);
+  }
+  float4* dst = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * N + col);
+  dst[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+  dst[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
 }  // namespace fvb
 
 using namespace fvb;
@@ -908,5 +952,25 @@ extern "C" int fvb_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const 
     rmsnorm_bwd_dw_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace, ctas, D, reinterpret_cast<__nv_bfloat16*>(dw));
     FVB_CHECK_CUDA(cudaGetLastError());
   }
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_bias_grad_bf16_workspace_bytes(int M, int N) {
+  return int64_t(std::max(1, std::min(M, BG_PARTS))) * std::max(N, 0) * 4;
+}
+
+extern "C" int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float* workspace, int64_t workspace_bytes, int M, int N,
+                                  void* stream) {
+  FVB_CHECK_ARG(dy && db && workspace, "null pointer");
+  FVB_CHECK_ARG(M > 0 && N > 0 && N % 8 == 0, "N must be a positive multiple of 8");
+  FVB_CHECK_ARG(lddy % 8 == 0, "lddy must be a multiple of 8");
+  FVB_CHECK_ARG(workspace_bytes >= fvb_bias_grad_bf16_workspace_bytes(M, N), "workspace too small");
+  const int parts = std::min(M, BG_PARTS);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  bias_grad_kernel<<<dim3(parts, (N / 8 + BG_THREADS - 1) / BG_THREADS), BG_THREADS, 0, st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(dy), lddy, workspace, M, N, parts);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  rmsnorm_bwd_dw_kernel<<<(N + 255) / 256, 256, 0, st>>>(workspace, parts, N, reinterpret_cast<__nv_bfloat16*>(db));
+  FVB_CHECK_CUDA(cudaGetLastError());
   return FVB_OK;
 }

@@ -14,6 +14,11 @@
 // The int8 x int8 path (I8, W8A8) loads both operands like the fp8 path (128-element k-blocks, 128B swizzle) and runs
 // s8 MMAs into s32 accumulators. |acc| <= 127^2 K fits in s32 for K <= FVB_I8_MAX_K, so the sums are exact and need no
 // promotion registers: the tile widths and the one-k-block-in-flight mainloop are the bf16 path's.
+// Transposed operands (TA / TB, bf16 only: the backward of the bf16 linear): an MN-major operand is stored [K][MN] with MN
+// contiguous and lands as 64-element x 64-row TMA boxes (128B swizzle), one 8 KB box per 64-wide MN chunk, chunk-major in
+// the stage, so a stage holds the same bytes as the K-major tile. wgmma reads it with imm-trans set:
+//   dgrad dx[M,K] = dy[M,N] . w[N,K]  -> A = dy (K-major), B = w (MN-major)              (TB)
+//   wgrad dw[N,K] = dy^T . x           -> A = dy^T (MN-major), B = x (MN-major), over M  (TA, TB)
 //
 // Stands behind fastvideo/layers/linear.py:146-156 (F.linear) and the elementwise op that follows
 // each linear in fastvideo/models/dits/wanvideo.py:394-431; rounding points mirror the reference's
@@ -38,6 +43,8 @@ constexpr int GEMM_BK_FP8 = 128;  // 128 e4m3 / int8 = one 128B swizzle row
 constexpr int FVB_I8_MAX_K = 133144;  // 127^2 * 133144 < 2^31
 constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_GROUP_M = 8;
+constexpr int GEMM_MN_CHUNK = 64;                         // MN-major operands: elements per 128B swizzle row
+constexpr int GEMM_MN_CHUNK_BYTES = GEMM_MN_CHUNK * GEMM_BK * 2;  // one 64 x 64 bf16 box: 8 KB
 
 struct GemmParams {
   const __nv_bfloat16* bias;
@@ -170,10 +177,13 @@ FVB_DEVICE void w8_widen_tile(uint32_t sb, int t) {
 FVB_DEVICE float acc_f32(float v) { return v; }
 FVB_DEVICE float acc_f32(int32_t v) { return __int2float_rn(v); }
 
-// FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); I8: int8 x int8 (W8A8); none: bf16 x bf16
-template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false>
+// FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); I8: int8 x int8 (W8A8); none: bf16 x bf16.
+// TA / TB: A / B is MN-major (bf16 x bf16 only).
+template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false, bool TA = false, bool TB = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8 || W8 || I8> p) {
+  static_assert(!((TA || TB) && (FP8 || W8 || I8)), "transposed operands are bf16 only: e4m3 / s8 wgmma has no transpose bits");
+  static_assert(TB || !TA, "the transposed producer loads B MN-major: TA comes with TB (wgrad)");
   using Cfg = GemmCfg<BN>;
   constexpr int BK = FP8 || I8 ? GEMM_BK_FP8 : GEMM_BK;
   using Acc = std::conditional_t<I8, int32_t, float>;
@@ -233,6 +243,39 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (++stage == Cfg::STAGES) {
             stage = 0;
             phase ^= 1;
+          }
+        }
+      }
+      return;
+    }
+    if constexpr (TA || TB) {
+      // MN-major operands: one 2-D TMA per 64-wide chunk ([K][MN] maps; MN and K tails zero-filled), chunk-major in the stage.
+      // A K-major A (TB only) is the forward's 4-D load.
+      if (threadIdx.x == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          int m_blk, n_blk;
+          tile_coords(tile, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
+          for (int kb = 0; kb < p.num_k; ++kb) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+            uint8_t* sb = sa + Cfg::A_BYTES;
+            mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+            if constexpr (TA) {
+#pragma unroll
+              for (int c = 0; c < GEMM_BM / GEMM_MN_CHUNK; ++c)
+                tma_load_2d(sa + c * GEMM_MN_CHUNK_BYTES, &tmA, &full[stage], m_blk * GEMM_BM + c * GEMM_MN_CHUNK, kb * BK);
+            } else {
+              tma_load_4d(sa, &tmA, &full[stage], kb * BK, m_blk * GEMM_BM, 0, 0);
+            }
+#pragma unroll
+            for (int c = 0; c < BN / GEMM_MN_CHUNK; ++c)
+              tma_load_2d(sb + c * GEMM_MN_CHUNK_BYTES, &tmB, &full[stage], n_blk * BN + c * GEMM_MN_CHUNK, kb * BK);
+            if (++stage == Cfg::STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
           }
         }
       }
@@ -317,6 +360,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if constexpr (I8) {
 #pragma unroll
         for (int k = 0; k < GEMM_BK_FP8 / 32; ++k) wgmma_ss_s8<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), 1);
+      } else if constexpr (TA || TB) {
+        // MN-major: this warpgroup's 64 A rows are chunk `half` (the same +8 KB as the K-major half); chunks are 8 KB apart
+        // (LBO), 8-row k groups 1024 B (SBO); a k16 step is 16 rows of 128 B (+128 on the descriptor)
+        const uint64_t ta = TA ? make_desc_mnmajor_sw128(sa, GEMM_MN_CHUNK_BYTES) : da;
+        const uint64_t tb = TB ? make_desc_mnmajor_sw128(sb, GEMM_MN_CHUNK_BYTES) : db;
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k)
+          wgmma_ss_trans<BN, TA, TB>(acc, ta + uint64_t(k * (TA ? 128 : 2)), tb + uint64_t(k * (TB ? 128 : 2)));
       } else {
 #pragma unroll
         for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k));
@@ -414,10 +465,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
-template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false>
+template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false, bool TA = false, bool TB = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsT<FP8 || W8 || I8>& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_kernel<BN, EPI, FP8, W8, I8>;
+  auto kern = gemm_kernel<BN, EPI, FP8, W8, I8, TA, TB>;
   static bool configured = false;
   if (!configured) {
     FVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -650,4 +701,79 @@ extern "C" int fvb_linear_w8a8_sp(const void* xq, int64_t ldx, const float* x_sc
   if (out_col_offsets != nullptr && N % 128 != 0) return set_error(FVB_ERR_INVALID_ARG, "column-block offsets need N %% 128 == 0%s");
   return gemm_impl(xq, ldx, 0, 0, 0, wq, ldw, 0, bias, out, ldo, 0, out_col_offsets, resid, ldr, gate, gate_rows, gate_stride,
                    1.0f, M, N, K, 1, epilogue, stream, x_scale, w_scale, true);
+}
+
+// ------------------------------------------------------------------------------------------------------------------------
+// Backward of the bf16 linear y = x w^T + b (fvb_linear_dgrad_bf16 / fvb_linear_wgrad_bf16; arithmetic in include/fvb200.h).
+// out[Mo, No] = bf16(sum_r A(mo, r) * B(r, no)) with fp32 accumulation, the plain FVB_EPI_BIAS store without bias. A is
+// K-major [Mo][R] (a_mn_major = false) or MN-major [R][Mo] (true); B is always MN-major [R][No]. R tails are zero-filled by
+// TMA, Mo tails are the epilogue's row check; No must be a multiple of 8 (whole bf16x2 column pairs, 16-byte rows).
+// No split-K: every output element is one CTA's sum in k-block order, so two calls give the same bits.
+// ------------------------------------------------------------------------------------------------------------------------
+template <bool TA>
+static int dispatch_bwd(int BN, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, cudaStream_t st) {
+  if (BN == 256) return launch_gemm<256, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
+  if (BN == 128) return launch_gemm<128, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
+  return launch_gemm<64, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
+}
+
+static int gemm_bwd_impl(bool a_mn_major, const void* a, int64_t lda, const void* b, int64_t ldb, void* out, int64_t ldo,
+                         int Mo, int No, int R, bool weight_stripes, void* stream) {
+  FVB_CHECK_ARG(a && b && out, "null pointer");
+  FVB_CHECK_ARG(Mo > 0 && No > 0 && R > 0, "empty problem");
+  FVB_CHECK_ARG(No % 8 == 0, "output columns (K of the forward) must be a multiple of 8");
+  FVB_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0 && ldo % 8 == 0, "row strides must be multiples of 8");
+  FVB_CHECK_ARG(ldo >= No, "output row stride must cover the output columns");
+  const int BN = (No >= 256 && No % 256 == 0) ? 256 : (No >= 128 && No % 128 == 0 ? 128 : (No >= 192 ? 256 : 64));
+  // bind the device's primary context to this thread before the driver-API encode: autograd runs the backward on its own
+  // worker thread, where no runtime call may have made it current yet (the encode then fails with CUDA_ERROR_INVALID_CONTEXT)
+  FVB_CHECK_CUDA(cudaFree(nullptr));
+  CUtensorMap tmA, tmB;
+  if (a_mn_major) {
+    uint64_t dims[2] = {(uint64_t)Mo, (uint64_t)R};
+    uint64_t str[2] = {2, (uint64_t)lda * 2};
+    uint32_t box[2] = {(uint32_t)GEMM_MN_CHUNK, (uint32_t)GEMM_BK};
+    if (int r = make_tmap_bf16(&tmA, a, 2, dims, str, box)) return r;
+  } else {  // the forward's A map: [batch 1][segment 1][Mo][R]
+    uint64_t dims[4] = {(uint64_t)R, (uint64_t)Mo, 1, 1};
+    uint64_t str[4] = {2, (uint64_t)lda * 2, 32, 16};  // unused dimensions (size 1): any 16-byte multiple
+    uint32_t box[4] = {(uint32_t)GEMM_BK, GEMM_BM, 1, 1};
+    if (int r = make_tmap_bf16(&tmA, a, 4, dims, str, box)) return r;
+  }
+  {
+    uint64_t dims[2] = {(uint64_t)No, (uint64_t)R};
+    uint64_t str[2] = {2, (uint64_t)ldb * 2};
+    uint32_t box[2] = {(uint32_t)GEMM_MN_CHUNK, (uint32_t)GEMM_BK};
+    if (int r = make_tmap_bf16(&tmB, b, 2, dims, str, box)) return r;
+  }
+  GemmParams p{};
+  p.out = out;
+  p.ldo = ldo;
+  p.a_seg_len = R;
+  p.div = 1.f;
+  p.M = Mo;
+  p.N = No;
+  p.K = R;
+  p.batch = 1;
+  p.num_m = (Mo + GEMM_BM - 1) / GEMM_BM;
+  p.num_n = (No + BN - 1) / BN;
+  p.num_k = (R + GEMM_BK - 1) / GEMM_BK;
+  // dgrad: the forward's weight-stripe raster (a stripe of w's columns stays in L2 while dy streams past it). wgrad: the
+  // row-group raster -- the ~132 resident tiles cover 8 row-blocks x ~16 column tiles and walk the token axis in step, so
+  // each k-block of dy and x is read from HBM once per wave and shared through L2 by 16 resp. 8 CTAs.
+  p.stripe_n = weight_stripes && p.num_m >= 16 && p.num_n > 8 ? 8 : 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return a_mn_major ? dispatch_bwd<true>(BN, tmA, tmB, p, st) : dispatch_bwd<false>(BN, tmA, tmB, p, st);
+}
+
+extern "C" int fvb_linear_dgrad_bf16(const void* dy, int64_t lddy, const void* w, int64_t ldw, void* dx, int64_t lddx, int M,
+                                     int N, int K, void* stream) {
+  // dx[M, K] = dy[M, N] . w[N, K]: A = dy (K-major over n), B = w (MN-major: row n holds the K output columns)
+  return gemm_bwd_impl(false, dy, lddy, w, ldw, dx, lddx, M, K, N, true, stream);
+}
+
+extern "C" int fvb_linear_wgrad_bf16(const void* dy, int64_t lddy, const void* x, int64_t ldx, void* dw, int64_t lddw, int M,
+                                     int N, int K, void* stream) {
+  // dw[N, K] = dy^T . x over the M tokens: A = dy^T (MN-major: token row m holds the N output rows), B = x (MN-major)
+  return gemm_bwd_impl(true, dy, lddy, x, ldx, dw, lddw, N, K, M, false, stream);
 }

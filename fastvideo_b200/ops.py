@@ -60,6 +60,37 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, e
     return out.reshape(*x.shape[:-1], N)
 
 
+def linear_bwd(x: torch.Tensor, w: torch.Tensor, dy: torch.Tensor, need_dx: bool = True, need_dw: bool = True,
+               need_db: bool = False):
+    """Backward of y = linear(x, w, bias) (FVB_EPI_BIAS) on the bf16 wgmma GEMM: x [M, K], w [N, K], dy [M, N] bf16 2-D views
+    with unit inner stride (row strides multiples of 8: column slices of fused buffers are read in place); K a multiple of
+    8 for dx / dw, N for db. Returns (dx [M, K], dw [N, K], db [N]), each fp32-accumulated and rounded to bf16 once, with
+    None for what was not requested (and not launched): fvb_linear_dgrad_bf16, fvb_linear_wgrad_bf16, fvb_bias_grad_bf16."""
+    for n, t in (("x", x), ("w", w), ("dy", dy)):
+        _require_cuda_bf16(t, n)
+        if t.dim() != 2 or t.stride(1) != 1:
+            raise FvbError(f"linear_bwd: {n} must be a 2-D view with unit inner stride")
+    M, K = x.shape
+    N = w.shape[0]
+    if w.shape[1] != K or dy.shape != (M, N):
+        raise FvbError(f"linear_bwd: x [M, K], w [N, K], dy [M, N] (got {tuple(x.shape)}, {tuple(w.shape)}, {tuple(dy.shape)})")
+    dx = dw = db = None
+    if need_dx:
+        dx = torch.empty((M, K), dtype=torch.bfloat16, device=x.device)
+        check(lib().fvb_linear_dgrad_bf16(ptr(dy), c_int64(dy.stride(0)), ptr(w), c_int64(w.stride(0)), ptr(dx), c_int64(K),
+                                          c_int(M), c_int(N), c_int(K), stream_ptr()))
+    if need_dw:
+        dw = torch.empty((N, K), dtype=torch.bfloat16, device=x.device)
+        check(lib().fvb_linear_wgrad_bf16(ptr(dy), c_int64(dy.stride(0)), ptr(x), c_int64(x.stride(0)), ptr(dw), c_int64(K),
+                                          c_int(M), c_int(N), c_int(K), stream_ptr()))
+    if need_db:
+        db = torch.empty(N, dtype=torch.bfloat16, device=x.device)
+        ws = _workspace(int(lib().fvb_bias_grad_bf16_workspace_bytes(c_int(M), c_int(N))), x.device)
+        check(lib().fvb_bias_grad_bf16(ptr(dy), c_int64(dy.stride(0)), ptr(db), _f32p(ws), c_int64(ws.numel()), c_int(M),
+                                       c_int(N), stream_ptr()))
+    return dx, dw, db
+
+
 FP8_E4M3_MAX = 448.0
 
 

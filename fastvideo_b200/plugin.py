@@ -38,9 +38,11 @@ What install() registers, and the reference interface each piece stands behind:
                       to forward_cuda for the classes that got one.
   whole block         load_wan_block(): a reference WanTransformerBlock(_VSA)'s state_dict() -> wan_dit.WanBlock.
 
-Training: the dense backend (through B200AttentionImpl, backward fvb_attention_bwd) and RMSNorm.forward_cuda (backward
-fvb_rmsnorm_bwd) are differentiable when grad is enabled and an input requires grad; without grad they run the same
-calls as before. The VSA impl above, the 8-bit backend and the linear methods are forward-only.
+Training: the dense backend (through B200AttentionImpl, backward fvb_attention_bwd), RMSNorm.forward_cuda (backward
+fvb_rmsnorm_bwd) and the fvb200_bf16 linear method (through linear_forward, backward fvb_linear_dgrad_bf16 /
+fvb_linear_wgrad_bf16 / fvb_bias_grad_bf16) are differentiable when grad is enabled and an input requires grad; without
+grad they run the same calls as before. The VSA impl above, the 8-bit backend and the FP8, INT8-weight and W8A8 linear
+methods are forward-only.
 
 There is no CPU fallback anywhere: with non-CUDA tensors these classes raise FvbError exactly like the rest of the
 package. uninstall() restores every patched attribute.
@@ -220,7 +222,8 @@ def _define():
 
     # ------------------------------------------------------------------ linear
     class Fvb200LinearMethod(LinearMethodBase):
-        """UnquantizedLinearMethod's weight layout (layers/linear.py:120-156), applied by fvb_linear_bf16."""
+        """UnquantizedLinearMethod's weight layout (layers/linear.py:120-156), applied by linear_forward (fvb_linear_bf16;
+        differentiable when the input, the weight or the bias requires grad)."""
 
         def create_weights(self, layer, input_size_per_partition, output_partition_sizes, input_size, output_size,
                            params_dtype, **extra_weight_attrs) -> None:
@@ -231,16 +234,7 @@ def _define():
             set_weight_attrs(weight, extra_weight_attrs)
 
         def apply(self, layer, x, bias=None):
-            if not x.is_cuda:
-                raise FvbError("fvb200_bf16 linear needs CUDA tensors (there is no CPU fallback)")
-            w = layer.weight
-            if w.dtype != torch.bfloat16 or x.dtype != torch.bfloat16:
-                raise FvbError(f"fvb200_bf16 linear is bf16 x bf16 (got x {x.dtype}, weight {w.dtype})")
-            x2 = x.reshape(-1, x.shape[-1])
-            if x2.stride(-1) != 1:
-                x2 = x2.contiguous()
-            b = None if bias is None else bias.to(torch.bfloat16)
-            return ops.linear(x2, w, b).reshape(*x.shape[:-1], w.shape[0])
+            return linear_forward(x, layer.weight, bias)
 
     class Fvb200Bf16Config(QuantizationConfig):
         def get_name(self):
@@ -360,6 +354,45 @@ def _define():
         Fvb200Int8WeightLinearMethod=Fvb200Int8WeightLinearMethod, Fvb200Int8WeightConfig=Fvb200Int8WeightConfig,
         Fvb200W8A8LinearMethod=Fvb200W8A8LinearMethod, Fvb200W8A8Config=Fvb200W8A8Config)
     return ns
+
+
+def linear_forward(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None) -> torch.Tensor:
+    """Fvb200LinearMethod.apply (UnquantizedLinearMethod's F.linear, layers/linear.py:146-156): bf16(x w^T + bias) over the
+    last axis of x on fvb_linear_bf16. With grad enabled and x, w or bias requiring grad it runs _LinearFn (the same
+    forward call, backward on fvb_linear_dgrad_bf16 / fvb_linear_wgrad_bf16 / fvb_bias_grad_bf16); otherwise the plain call."""
+    if not x.is_cuda:
+        raise FvbError("fvb200_bf16 linear needs CUDA tensors (there is no CPU fallback)")
+    if w.dtype != torch.bfloat16 or x.dtype != torch.bfloat16:
+        raise FvbError(f"fvb200_bf16 linear is bf16 x bf16 (got x {x.dtype}, weight {w.dtype})")
+    x2 = x.reshape(-1, x.shape[-1])
+    if x2.stride(-1) != 1:
+        x2 = x2.contiguous()
+    b = None if bias is None else bias.to(torch.bfloat16)
+    if torch.is_grad_enabled() and (x.requires_grad or w.requires_grad or (b is not None and b.requires_grad)):
+        out = _LinearFn.apply(x2, w, b)
+    else:
+        out = ops.linear(x2, w, b)
+    return out.reshape(*x.shape[:-1], w.shape[0])
+
+
+class _LinearFn(torch.autograd.Function):
+    """y = bf16(x w^T + b) over rows of x [M, K], w bf16 [N, K], b bf16 [N] or None: forward on fvb_linear_bf16 (the output
+    of the no-grad call, bit for bit), backward on ops.linear_bwd for the inputs that need a gradient (nothing else is
+    launched). An fp32 bias is cast outside, so torch differentiates the cast."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        ctx.save_for_backward(x, w)
+        return ops.linear(x, w, b)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        dy = dy.to(torch.bfloat16)
+        if dy.stride(1) != 1 or dy.stride(0) % 8 != 0:
+            dy = dy.contiguous()
+        need_dx, need_dw, need_db = ctx.needs_input_grad
+        return ops.linear_bwd(x, w, dy, need_dx, need_dw, need_db)
 
 
 def rms_norm_forward_cuda(self, x: torch.Tensor, residual: torch.Tensor | None = None):
@@ -552,6 +585,6 @@ def uninstall() -> None:
     _state = None
 
 
-__all__ = ["available", "install", "uninstall", "load_wan_block", "rms_norm_forward_cuda", "route_dense", "DENSE_BACKEND_NAME",
+__all__ = ["available", "install", "uninstall", "load_wan_block", "linear_forward", "rms_norm_forward_cuda", "route_dense", "DENSE_BACKEND_NAME",
            "DENSE_8BIT_BACKEND_NAME", "QUANT_NAME", "QUANT_NAME_FP8",
            "QUANT_NAME_INT8W"]

@@ -81,6 +81,29 @@ int fvb_linear_bf16_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_
                        int epilogue, void* stream);
 
 /* --------------------------------------------------------------------------------------------
+ * Backward of the bf16 linear y = bf16(x w^T + b) (FVB_EPI_BIAS), for training. M, N, K keep the forward's meaning:
+ * x [M, K], w [N, K], dy [M, N], all bf16 with unit inner stride and row strides (ldx, ldw, lddy, lddx, lddw; multiples of
+ * 8) so column slices of fused buffers work in place. Each output is fp32-accumulated and rounded to bf16 once -- torch's
+ * rounding points for bf16 F.linear autograd. No split-K and no atomics: two calls give the same bits.
+ *
+ * fvb_linear_dgrad_bf16:  dx[m, k] = bf16(sum_n dy[m, n] * w[n, k])      K a multiple of 8 (dx's columns)
+ * fvb_linear_wgrad_bf16:  dw[n, k] = bf16(sum_m dy[m, n] * x[m, k])      K a multiple of 8 (dw's columns)
+ *   Both run the forward's wgmma GEMM with MN-major (transposed) shared-memory operands; reduction tails (N for dgrad, M
+ *   for wgrad) are zero-filled on load. Only [0, M) x [0, K) of dx and [0, N) x [0, K) of dw are written.
+ * fvb_bias_grad_bf16:     db[n] = bf16(sum_m float(dy[m, n]))             N a multiple of 8
+ *   Deterministic: each of min(M, 256) row sets (rows p, p + 256, ...) is summed in row order into an fp32 partial per
+ *   column, then the partials are added in row-set order and rounded once. workspace: device memory of
+ *   fvb_bias_grad_bf16_workspace_bytes(M, N) bytes, 16-byte aligned.
+ * -------------------------------------------------------------------------------------------- */
+int fvb_linear_dgrad_bf16(const void* dy, int64_t lddy, const void* w, int64_t ldw, void* dx, int64_t lddx, int M, int N, int K,
+                          void* stream);
+int fvb_linear_wgrad_bf16(const void* dy, int64_t lddy, const void* x, int64_t ldx, void* dw, int64_t lddw, int M, int N, int K,
+                          void* stream);
+int64_t fvb_bias_grad_bf16_workspace_bytes(int M, int N);
+int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float* workspace, int64_t workspace_bytes, int M, int N,
+                       void* stream);
+
+/* --------------------------------------------------------------------------------------------
  * FP8 (e4m3) linear layers: row-quantised activations x per-output-channel-quantised weights
  * Stands behind FastVideo's FP8 linear (fastvideo/layers/fp8linear.py, fastvideo/layers/quantization/) with this
  * library's own arithmetic, below.
