@@ -159,10 +159,27 @@ def compute_topk(sparsity: float, num_blocks: int) -> int:
     return max(1, min(math.ceil((1 - sparsity) * num_blocks), num_blocks))
 
 
+class _PermuteRowsFn(torch.autograd.Function):
+    """ops.gather_rows of [B, S, W] rows by a permutation table; the backward gathers the gradient with the inverse table."""
+
+    @staticmethod
+    def forward(ctx, x, idx, inv):
+        ctx.save_for_backward(inv)
+        return ops.gather_rows(x, idx)
+
+    @staticmethod
+    def backward(ctx, g):
+        inv, = ctx.saved_tensors
+        return ops.gather_rows(g.to(torch.bfloat16).contiguous(), inv), None, None
+
+
 class VideoSparseAttentionImpl:
     """VideoSparseAttentionImpl (video_sparse_attn.py:238-342). preprocess_qkv tiles the stacked [4B, S, H, d] tensor,
     forward runs VSA, postprocess_output untiles. Here "tiling" is a pure permutation into COMPACT tile-major order
-    (no zero-padded rows: the kernels mask by variable block size), done by one gather kernel."""
+    (no zero-padded rows: the kernels mask by variable block size), done by one gather kernel.
+    Differentiable: with grad enabled and an input that requires grad, tile / untile are autograd permutations (the
+    backward gathers with the inverse table) and forward runs vsa._VideoSparseAttnFn in the compact layout, whose output
+    is the no-grad call's, bit for bit."""
 
     def __init__(self, num_heads: int, head_size: int, causal: bool = False, softmax_scale: float | None = None,
                  num_kv_heads: int | None = None, prefix: str = "", **extra_impl_args) -> None:
@@ -170,13 +187,19 @@ class VideoSparseAttentionImpl:
             raise ValueError(f"libfvb200 VSA supports head_size 128, got {head_size}")
         self.prefix = prefix
 
-    def tile(self, x: torch.Tensor, md: VideoSparseAttentionMetadata) -> torch.Tensor:
+    @staticmethod
+    def _permute(x: torch.Tensor, idx: torch.Tensor, inv: torch.Tensor) -> torch.Tensor:
         B, S, H, d = x.shape
-        return ops.gather_rows(x.reshape(B, S, H * d), md.tile_partition_indices).view(B, S, H, d)
+        x3 = x.reshape(B, S, H * d)
+        if torch.is_grad_enabled() and x.requires_grad:
+            return _PermuteRowsFn.apply(x3, idx, inv).view(B, S, H, d)
+        return ops.gather_rows(x3, idx).view(B, S, H, d)
+
+    def tile(self, x: torch.Tensor, md: VideoSparseAttentionMetadata) -> torch.Tensor:
+        return self._permute(x, md.tile_partition_indices, md.reverse_tile_partition_indices)
 
     def untile(self, x: torch.Tensor, md: VideoSparseAttentionMetadata) -> torch.Tensor:
-        B, S, H, d = x.shape
-        return ops.gather_rows(x.reshape(B, S, H * d), md.reverse_tile_partition_indices).view(B, S, H, d)
+        return self._permute(x, md.reverse_tile_partition_indices, md.tile_partition_indices)
 
     def preprocess_qkv(self, qkv: torch.Tensor, attn_metadata: VideoSparseAttentionMetadata) -> torch.Tensor:
         return self.tile(qkv, attn_metadata)
@@ -188,6 +211,10 @@ class VideoSparseAttentionImpl:
                 attn_metadata: VideoSparseAttentionMetadata) -> torch.Tensor:
         md = attn_metadata
         topk = compute_topk(md.VSA_sparsity, md.variable_block_sizes.numel())
+        inputs = (query, key, value) if gate_compress is None else (query, key, value, gate_compress)
+        if torch.is_grad_enabled() and any(t.requires_grad for t in inputs):
+            return vsa._VideoSparseAttnFn.apply(query, key, value, gate_compress, md.variable_block_sizes, topk, None,
+                                                md.block_offsets, md.row_block)
         return vsa.video_sparse_attn_bshd(query, key, value, md.variable_block_sizes, topk, gate=gate_compress,
                                           block_off=md.block_offsets, row_block=md.row_block)
 

@@ -14,6 +14,8 @@
 // (kv block, head) for dK / dV walking the kv->q list; K/V (resp. Q/dO) tiles staged through shared memory.
 #include <mma.h>
 
+#include <type_traits>
+
 #include "fvb_host.cuh"
 #include "fvb_ptx.cuh"
 
@@ -280,6 +282,15 @@ __global__ void __launch_bounds__(BW_THREADS) bwd_dkdv_kernel(BwdParams p) {
 // Warp roles as in the forward: warpgroup 0 is the producer (one TMA warp; setmaxnreg 24), warpgroups 1 and 2 consume
 // (setmaxnreg 240: the KV kernel holds two 64 x 128 fp32 accumulators next to the 64 x 64 S^T and dP^T).
 // Keys >= Skv get P = 0 explicitly (TMA zero fill gives S = 0 there, and exp2(0 - lse) is not 0).
+//
+// Block-list mode (LIST = true, fvb_attention_sparse_bwd), same arithmetic: the two owned 64-row boxes are tiles 2 x and
+// 2 x + 1 of their layout, and the CTA walks the ascending union of those tiles' two lists (KV: kv -> q lists, else q -> kv),
+// merged on the fly as the forward merges its q-block lists (KeyWalk mode 2). Only the producer walks: with each stage it
+// publishes the item (2-bit "which warpgroup takes part" flags, the walked tile's valid rows) in shared memory, and after the
+// last one an end marker. A warpgroup whose flag bit is clear does no MMA for the item and only releases the stage. Tile i starts at row off[i] (64 i without off) and has len[i] valid rows
+// (the forward's rule, tile_rows); a box starting there also reads the next tile's first rows, so keys past the walked kv
+// tile's length get P = 0, q rows past the walked q tile's length get lse = +inf / delta = 0 (KV) or are not loaded (dQ), and
+// the epilogue stores only the owned tile's valid rows.
 constexpr int DB_THREADS = 384;
 constexpr int DB_STAGES = 3;
 constexpr int DB_TILE = 64 * 128 * 2;  // 16 KB: [d half (2)][64 rows][128 B], the forward's tile
@@ -296,11 +307,39 @@ struct DenseBwdParams {
   float scale, scale_log2;
 };
 
+struct SparseBwdParams : DenseBwdParams {
+  const int32_t *list_idx, *list_num;     // KV: k2q lists, else q2k: [B?, H?, n_own, cap] ascending / [.., n_own]
+  int64_t list_stride_b, list_stride_h;   // in list rows (0 = broadcast)
+  int cap, n_own;
+  const int32_t *own_off, *own_len;       // tiles a CTA owns (KV: kv tiles, else q tiles); NULL = the padded rule
+  const int32_t *walk_off, *walk_len;     // tiles it walks (KV: q tiles, else kv tiles)
+};
+
+// first row and valid rows of tile i, the forward's rule: row0 = off[i] (64 i without off), rows = len[i] (without len:
+// off[i + 1] - off[i], else 64), at most 64 and never past S
+FVB_DEVICE void tile_rows(const int32_t* off, const int32_t* len, int i, int S, int& row0, int& rows) {
+  row0 = off ? __ldg(off + i) : 64 * i;
+  const int l = len ? __ldg(len + i) : (off ? __ldg(off + i + 1) - row0 : 64);
+  rows = min(min(l, 64), max(0, S - row0));
+}
+
+// owned tile s of the CTA (block-list mode): its first row and valid rows; a missing second tile has none
 template <bool KV>
+FVB_DEVICE void own_tile(const SparseBwdParams& p, int s, int& row0, int& rows) {
+  const int t = 2 * blockIdx.x + s, S = KV ? p.Skv : p.Sq;
+  if (t < p.n_own) {
+    tile_rows(p.own_off, p.own_len, t, S, row0, rows);
+  } else {
+    row0 = S;
+    rows = 0;
+  }
+}
+
+template <bool KV, bool LIST>
 __global__ void __launch_bounds__(DB_THREADS, 1)
 attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                       const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                      const DenseBwdParams p) {
+                      const std::conditional_t<LIST, SparseBwdParams, DenseBwdParams> p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // resident: [warpgroup (2)][operand (2)][tile] -- KV: (K, V), else (Q, dO); ring: [stage][operand (2)][tile] -- KV:
@@ -312,6 +351,7 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   uint64_t* res_full = reinterpret_cast<uint64_t*>(sDelta + DB_STAGES * 64);
   uint64_t* full = res_full + 1;
   uint64_t* empty = full + DB_STAGES;
+  // LIST: int [stage] after the barriers, the walk item of each stage: flags | walked rows << 2, or -1 = end of walk
 
   const int h = blockIdx.y, b = blockIdx.z;
   const int n_walk = KV ? (p.Sq + 63) / 64 : (p.Skv + 63) / 64;
@@ -341,20 +381,38 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
       mbar_expect_tx(res_full, 4 * DB_TILE);
       for (int s = 0; s < 2; ++s)
         for (int hf = 0; hf < 2; ++hf) {
-          const int row0 = (2 * blockIdx.x + s) * 64;
+          int row0 = (2 * blockIdx.x + s) * 64, rows;
+          if constexpr (LIST) own_tile<KV>(p, s, row0, rows);
           tma_load_4d(sRes + (2 * s) * DB_TILE + hf * DB_HALF, res0, res_full, hf * 64, row0, h, b);
           tma_load_4d(sRes + (2 * s + 1) * DB_TILE + hf * DB_HALF, res1, res_full, hf * 64, row0, h, b);
         }
     }
+    KeyWalk walk;  // LIST: the union of the two owned tiles' lists
+    if constexpr (LIST) {
+      const int64_t r0 = int64_t(b) * p.list_stride_b + int64_t(h) * p.list_stride_h + 2 * blockIdx.x;
+      walk.mode = 2;
+      walk.i0 = walk.i1 = 0;
+      walk.l0 = p.list_idx + r0 * p.cap;
+      walk.l1 = walk.l0 + p.cap;
+      walk.n0 = min(__ldg(p.list_num + r0), p.cap);
+      walk.n1 = 2 * int(blockIdx.x) + 1 < p.n_own ? min(__ldg(p.list_num + r0 + 1), p.cap) : 0;
+    }
     int stage = 0;
     uint32_t phase = 0;
-    for (int t = 0; t < n_walk; ++t) {
+    int flags;
+    for (int t = 0; LIST ? walk.next(t, flags) : t < n_walk; ++t) {  // LIST: next() sets t
       mbar_wait(&empty[stage], phase ^ 1);
+      int row0 = t * 64, rows = 64;
+      if constexpr (LIST) {
+        tile_rows(p.walk_off, p.walk_len, t, KV ? p.Sq : p.Skv, row0, rows);
+        if (lane == 0) reinterpret_cast<int*>(empty + DB_STAGES)[stage] = flags | rows << 2;
+      }
       if constexpr (KV) {
         for (int r = lane; r < 64; r += 32) {
-          const int q = t * 64 + r;
-          sLse[stage * 64 + r] = q < p.Sq ? __ldg(p.lse + int64_t(b) * p.lse_stride_b + int64_t(h) * p.lse_stride_h + q) : INFINITY;
-          sDelta[stage * 64 + r] = q < p.Sq ? __ldg(p.delta + bh * p.Sq + q) : 0.f;
+          const int q = row0 + r;
+          const bool valid = LIST ? r < rows : q < p.Sq;
+          sLse[stage * 64 + r] = valid ? __ldg(p.lse + int64_t(b) * p.lse_stride_b + int64_t(h) * p.lse_stride_h + q) : INFINITY;
+          sDelta[stage * 64 + r] = valid ? __ldg(p.delta + bh * p.Sq + q) : 0.f;
         }
         __syncwarp();
       }
@@ -362,13 +420,20 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         uint8_t* dst = sRing + stage * 2 * DB_TILE;
         mbar_expect_tx(&full[stage], 2 * DB_TILE);  // also the arrive that publishes the staged lse / delta
         for (int hf = 0; hf < 2; ++hf) {
-          tma_load_4d(dst + hf * DB_HALF, ring0, &full[stage], hf * 64, t * 64, h, b);
-          tma_load_4d(dst + DB_TILE + hf * DB_HALF, ring1, &full[stage], hf * 64, t * 64, h, b);
+          tma_load_4d(dst + hf * DB_HALF, ring0, &full[stage], hf * 64, row0, h, b);
+          tma_load_4d(dst + DB_TILE + hf * DB_HALF, ring1, &full[stage], hf * 64, row0, h, b);
         }
       }
       if (++stage == DB_STAGES) {
         stage = 0;
         phase ^= 1;
+      }
+    }
+    if constexpr (LIST) {
+      mbar_wait(&empty[stage], phase ^ 1);
+      if (lane == 0) {
+        reinterpret_cast<int*>(empty + DB_STAGES)[stage] = -1;
+        mbar_arrive(&full[stage]);
       }
     }
     return;
@@ -378,8 +443,9 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   reg_alloc<240>();  // 128 x 24 + 256 x 240 = 64 512 of 65 536 registers
   const int s = wg - 1;
   const int tq = lane & 3;
-  const int own0 = (2 * blockIdx.x + s) * 64;
-  const int own_rows = max(0, min(64, (KV ? p.Skv : p.Sq) - own0));
+  int own0 = (2 * blockIdx.x + s) * 64;
+  int own_rows = max(0, min(64, (KV ? p.Skv : p.Sq) - own0));
+  if constexpr (LIST) own_tile<KV>(p, s, own0, own_rows);
   const uint32_t ra0 = smem_u32(sRes + (2 * s) * DB_TILE), ra1 = smem_u32(sRes + (2 * s + 1) * DB_TILE);
   // KV: lse / delta come per column from shared memory; else per row, from global once
   float row_lse[2] = {INFINITY, INFINITY}, row_delta[2] = {0.f, 0.f};
@@ -399,9 +465,14 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   mbar_wait(res_full, 0);
   int stage = 0;
   uint32_t phase = 0;
-  for (int t = 0; t < n_walk; ++t) {
+  for (int t = 0; LIST || t < n_walk; ++t) {  // LIST: until the end marker
     mbar_wait(&full[stage], phase);
-    if (own_rows > 0) {
+    int item = 3;
+    if constexpr (LIST) {
+      item = reinterpret_cast<const int*>(empty + DB_STAGES)[stage];
+      if (item < 0) break;
+    }
+    if (own_rows > 0 && (!LIST || ((item >> s) & 1))) {
       const uint32_t ga0 = smem_u32(sRing + stage * 2 * DB_TILE), ga1 = ga0 + DB_TILE;
       float sc[32], dp[32];  // KV: S^T, dP^T (rows = keys, columns = q rows); else S, dP
 #pragma unroll
@@ -422,7 +493,7 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
       wgmma_fence_regs(sc);
       wgmma_fence_regs(dp);
       // P = exp2(S scale log2e - lse), dS = P (dP - delta) scale on rows (16 warp + lane / 4 + 8 i), columns (8 j + 2 tq + c)
-      const int col_valid = KV ? 64 : min(64, p.Skv - t * 64);
+      const int col_valid = KV ? 64 : LIST ? item >> 2 : min(64, p.Skv - t * 64);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float2 cl = make_float2(0.f, 0.f), cd = make_float2(0.f, 0.f);
@@ -501,6 +572,57 @@ attn_bwd_dense_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 
 using namespace fvb;
 
+// delta = rowsum(dO * O) (the block-list backward's row kernel), the four TMA maps and the parameters both wgmma backward
+// kernels share
+static int wgmma_bwd_setup(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
+                           int64_t lse_stride_b, int64_t lse_stride_h, float* delta_ws, const int64_t* const (&st8)[8], int B,
+                           int H, int Sq, int Skv, float softmax_scale, cudaStream_t st, CUtensorMap (&tm)[4],
+                           DenseBwdParams& p) {
+  for (auto s : st8)
+    for (int i = 0; i < 3; ++i) FVB_CHECK_ARG(s[i] % 8 == 0, "strides must be multiples of 8 elements");
+  auto S3 = [](const int64_t* s) { return BwdStr{s[0], s[1], s[2]}; };
+  BwdParams dp = {};
+  dp.o = reinterpret_cast<const __nv_bfloat16*>(o);
+  dp.dO = reinterpret_cast<const __nv_bfloat16*>(dO);
+  dp.so = S3(st8[3]);
+  dp.sdo = S3(st8[4]);
+  dp.delta = delta_ws;
+  dp.Sq = Sq;
+  dp.H = H;
+  const int64_t rows = int64_t(B) * H * Sq;
+  bwd_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(dp, B);
+  FVB_CHECK_CUDA(cudaGetLastError());
+
+  int r;
+  if ((r = make_qkv_tmap(&tm[0], q, Sq, H, B, st8[0][1], st8[0][2], st8[0][0]))) return r;
+  if ((r = make_qkv_tmap(&tm[1], k, Skv, H, B, st8[1][1], st8[1][2], st8[1][0]))) return r;
+  if ((r = make_qkv_tmap(&tm[2], v, Skv, H, B, st8[2][1], st8[2][2], st8[2][0]))) return r;
+  if ((r = make_qkv_tmap(&tm[3], dO, Sq, H, B, st8[4][1], st8[4][2], st8[4][0]))) return r;
+  p = {};
+  p.lse = lse;
+  p.lse_stride_b = lse_stride_b;
+  p.lse_stride_h = lse_stride_h;
+  p.delta = delta_ws;
+  p.Sq = Sq;
+  p.Skv = Skv;
+  p.H = H;
+  p.scale = softmax_scale;
+  p.scale_log2 = softmax_scale * 1.4426950408889634f;
+  return FVB_OK;
+}
+
+template <bool KV, bool LIST, typename P>
+static int launch_wgmma_bwd(const CUtensorMap (&tm)[4], const P& p, int n_own, int H, int B, cudaStream_t st) {
+  static bool configured = false;
+  if (!configured) {
+    FVB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dense_kernel<KV, LIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_SMEM));
+    configured = true;
+  }
+  attn_bwd_dense_kernel<KV, LIST><<<dim3((n_own + 1) / 2, H, B), DB_THREADS, DB_SMEM, st>>>(tm[0], tm[1], tm[2], tm[3], p);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
 extern "C" int fvb_attention_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
                                  int64_t lse_stride_b, int64_t lse_stride_h, void* dq, void* dk, void* dv, float* delta_ws,
                                  const int64_t* q_strides, const int64_t* k_strides, const int64_t* v_strides,
@@ -511,58 +633,85 @@ extern "C" int fvb_attention_bwd(const void* q, const void* k, const void* v, co
   FVB_CHECK_ARG(head_dim == 128, "head_dim must be 128");
   FVB_CHECK_ARG(B > 0 && H > 0 && Sq > 0 && Skv > 0, "empty problem");
   FVB_CHECK_ARG(H <= 65535 && B <= 65535, "too many heads / batches");
-  const int64_t* all[8] = {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides};
-  for (auto st : all)
-    for (int i = 0; i < 3; ++i) FVB_CHECK_ARG(st[i] % 8 == 0, "strides must be multiples of 8 elements");
-  auto S3 = [](const int64_t* s) { return BwdStr{s[0], s[1], s[2]}; };
+  const int64_t* const all[8] = {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides};
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // delta = rowsum(dO * O), the block-list backward's row kernel
-  BwdParams dp = {};
-  dp.o = reinterpret_cast<const __nv_bfloat16*>(o);
-  dp.dO = reinterpret_cast<const __nv_bfloat16*>(dO);
-  dp.so = S3(o_strides);
-  dp.sdo = S3(do_strides);
-  dp.delta = delta_ws;
-  dp.Sq = Sq;
-  dp.H = H;
-  const int64_t rows = int64_t(B) * H * Sq;
-  bwd_delta_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(dp, B);
-  FVB_CHECK_CUDA(cudaGetLastError());
-
-  CUtensorMap tmQ, tmK, tmV, tmdO;
+  CUtensorMap tm[4];
+  DenseBwdParams p;
   int r;
-  if ((r = make_qkv_tmap(&tmQ, q, Sq, H, B, q_strides[1], q_strides[2], q_strides[0]))) return r;
-  if ((r = make_qkv_tmap(&tmK, k, Skv, H, B, k_strides[1], k_strides[2], k_strides[0]))) return r;
-  if ((r = make_qkv_tmap(&tmV, v, Skv, H, B, v_strides[1], v_strides[2], v_strides[0]))) return r;
-  if ((r = make_qkv_tmap(&tmdO, dO, Sq, H, B, do_strides[1], do_strides[2], do_strides[0]))) return r;
-  DenseBwdParams p = {};
-  p.lse = lse;
-  p.lse_stride_b = lse_stride_b;
-  p.lse_stride_h = lse_stride_h;
-  p.delta = delta_ws;
-  p.Sq = Sq;
-  p.Skv = Skv;
-  p.H = H;
-  p.scale = softmax_scale;
-  p.scale_log2 = softmax_scale * 1.4426950408889634f;
-  static bool configured = false;
-  if (!configured) {
-    FVB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dense_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_SMEM));
-    FVB_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dense_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DB_SMEM));
-    configured = true;
-  }
+  if ((r = wgmma_bwd_setup(q, k, v, o, dO, lse, lse_stride_b, lse_stride_h, delta_ws, all, B, H, Sq, Skv, softmax_scale, st, tm, p)))
+    return r;
+  auto S3 = [](const int64_t* s) { return BwdStr{s[0], s[1], s[2]}; };
   p.out0 = reinterpret_cast<__nv_bfloat16*>(dk);
   p.out1 = reinterpret_cast<__nv_bfloat16*>(dv);
   p.so0 = S3(dk_strides);
   p.so1 = S3(dv_strides);
-  attn_bwd_dense_kernel<true><<<dim3((Skv + 127) / 128, H, B), DB_THREADS, DB_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
-  FVB_CHECK_CUDA(cudaGetLastError());
+  if ((r = launch_wgmma_bwd<true, false>(tm, p, (Skv + 63) / 64, H, B, st))) return r;
   p.out0 = reinterpret_cast<__nv_bfloat16*>(dq);
   p.out1 = nullptr;
   p.so0 = S3(dq_strides);
-  attn_bwd_dense_kernel<false><<<dim3((Sq + 127) / 128, H, B), DB_THREADS, DB_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
-  FVB_CHECK_CUDA(cudaGetLastError());
-  return FVB_OK;
+  return launch_wgmma_bwd<false, false>(tm, p, (Sq + 63) / 64, H, B, st);
+}
+
+extern "C" int fvb_attention_sparse_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO,
+                                        const float* lse, int64_t lse_stride_b, int64_t lse_stride_h, void* dq, void* dk,
+                                        void* dv, float* delta_ws, const int64_t* q_strides, const int64_t* k_strides,
+                                        const int64_t* v_strides, const int64_t* o_strides, const int64_t* do_strides,
+                                        const int64_t* dq_strides, const int64_t* dk_strides, const int64_t* dv_strides, int B,
+                                        int H, int Sq, int Skv, int head_dim, float softmax_scale, const int32_t* q2k_idx,
+                                        const int32_t* q2k_num, int capq, const int32_t* k2q_idx, const int32_t* k2q_num,
+                                        int capk, int64_t idx_stride_b, int64_t idx_stride_h, int64_t kidx_stride_b,
+                                        int64_t kidx_stride_h, const int32_t* q_off, const int32_t* q_len, int nqb,
+                                        const int32_t* kv_off, const int32_t* kv_len, int nkb, void* stream) {
+  FVB_CHECK_ARG(q && k && v && o && dO && lse && dq && dk && dv && delta_ws && q2k_idx && q2k_num && k2q_idx && k2q_num,
+                "null pointer");
+  FVB_CHECK_ARG(head_dim == 128, "head_dim must be 128");
+  FVB_CHECK_ARG(B > 0 && H > 0 && Sq > 0 && Skv > 0 && nqb > 0 && nkb > 0 && capq > 0 && capk > 0, "empty problem");
+  FVB_CHECK_ARG(H <= 65535 && B <= 65535, "too many heads / batches");
+  FVB_CHECK_ARG((idx_stride_h == 0 || idx_stride_h == nqb) &&
+                    (idx_stride_b == 0 || idx_stride_b == (idx_stride_h ? int64_t(H) * nqb : int64_t(nqb))),
+                "q2k index tensors must be contiguous [B or 1, H or 1, nqb, capq]");
+  FVB_CHECK_ARG((kidx_stride_h == 0 || kidx_stride_h == nkb) &&
+                    (kidx_stride_b == 0 || kidx_stride_b == (kidx_stride_h ? int64_t(H) * nkb : int64_t(nkb))),
+                "k2q index tensors must be contiguous [B or 1, H or 1, nkb, capk]");
+  const int64_t* const all[8] = {q_strides, k_strides, v_strides, o_strides, do_strides, dq_strides, dk_strides, dv_strides};
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUtensorMap tm[4];
+  SparseBwdParams p;
+  int r;
+  if ((r = wgmma_bwd_setup(q, k, v, o, dO, lse, lse_stride_b, lse_stride_h, delta_ws, all, B, H, Sq, Skv, softmax_scale, st, tm, p)))
+    return r;
+  auto S3 = [](const int64_t* s) { return BwdStr{s[0], s[1], s[2]}; };
+  // dK, dV: kv tiles owned, q tiles walked (the k2q lists)
+  p.out0 = reinterpret_cast<__nv_bfloat16*>(dk);
+  p.out1 = reinterpret_cast<__nv_bfloat16*>(dv);
+  p.so0 = S3(dk_strides);
+  p.so1 = S3(dv_strides);
+  p.list_idx = k2q_idx;
+  p.list_num = k2q_num;
+  p.list_stride_b = kidx_stride_b;
+  p.list_stride_h = kidx_stride_h;
+  p.cap = capk;
+  p.n_own = nkb;
+  p.own_off = kv_off;
+  p.own_len = kv_len;
+  p.walk_off = q_off;
+  p.walk_len = q_len;
+  if ((r = launch_wgmma_bwd<true, true>(tm, p, nkb, H, B, st))) return r;
+  // dQ: q tiles owned, kv tiles walked (the q2k lists)
+  p.out0 = reinterpret_cast<__nv_bfloat16*>(dq);
+  p.out1 = nullptr;
+  p.so0 = S3(dq_strides);
+  p.list_idx = q2k_idx;
+  p.list_num = q2k_num;
+  p.list_stride_b = idx_stride_b;
+  p.list_stride_h = idx_stride_h;
+  p.cap = capq;
+  p.n_own = nqb;
+  p.own_off = q_off;
+  p.own_len = q_len;
+  p.walk_off = kv_off;
+  p.walk_len = kv_len;
+  return launch_wgmma_bwd<false, true>(tm, p, nqb, H, B, st);
 }
 
 extern "C" int fvb_attention_blocklist_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO,

@@ -72,38 +72,7 @@ struct AttnSmem {
   static constexpr int BYTES = TILE * (2 + 2 * ATT_STAGES) + 1024 + 256;
 };
 
-// The CTA's walk over key blocks: next() yields (kv block, flags) in ascending order, flags bit s = q block s attends.
-// Every thread runs its own copy over the same global lists, so producer and consumers agree without communication.
-struct KeyWalk {
-  const int32_t* l0;
-  const int32_t* l1;
-  int n0, n1, i0, i1;
-  int mode;  // 0 dense, 1 pair list, 2 two q-block lists
-
-  FVB_DEVICE bool next(int& kb, int& flags) {
-    if (mode == 2) {
-      const int a = i0 < n0 ? __ldg(l0 + i0) : 0x7fffffff;
-      const int b = i1 < n1 ? __ldg(l1 + i1) : 0x7fffffff;
-      if (a == 0x7fffffff && b == 0x7fffffff) return false;
-      kb = min(a, b);
-      flags = (a == kb ? 1 : 0) | (b == kb ? 2 : 0);
-      i0 += a == kb;
-      i1 += b == kb;
-      return true;
-    }
-    if (i0 >= n0) return false;
-    if (mode == 0) {
-      kb = i0++;
-      flags = 3;
-      return true;
-    }
-    const int ent = __ldg(l0 + i0++);
-    kb = ent & 0xFFFFFF;
-    flags = (ent >> 24) & 3;
-    return true;
-  }
-};
-
+// The CTA's walk over key blocks (KeyWalk, fvb_ptx.cuh): flags bit s = q block s attends.
 FVB_DEVICE void kv_rows(const AttnParams& p, bool dense, int kb, int& row0, int& vlen) {
   if (dense) {
     row0 = kb * 64;

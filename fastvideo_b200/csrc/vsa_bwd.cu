@@ -7,6 +7,8 @@
 //   fvb_vsa_combine_bwd    d_gate = dO * out_c,  d_out_c = sum over a tile's valid rows of dO * gate (fixed order, fp32)
 //   fvb_softmax_rows_bwd   d_scores = attn * (d_attn - rowsum(d_attn * attn)) * scale, optionally with d_scores^T and attn^T
 //   fvb_block_mean_bwd     dx = dx_s + d_x_c / len on the valid rows, 0 on the pad rows
+// The *_compact variants (template flag COMPACT) take the compact layout instead: tile i is rows [off[i], off[i + 1]) of a
+// tile-major sequence without pad rows, so every row is a token and a tile's rows are never another tile's.
 #include "fvb_host.cuh"
 #include "fvb_ptx.cuh"
 
@@ -20,6 +22,8 @@ constexpr int VSA_TILE = 64;
 
 // One CTA (256 threads) per (tile, h, b). Thread t owns channels 8 (t & 15) .. +7 of rows t >> 4, +16, +32, +48; the 16 row
 // groups' partial sums are added in row-group order through shared memory, so the result does not depend on scheduling.
+// block_len is block_off [nblk + 1] when COMPACT; rows of the tile past its length are then neither read nor written.
+template <bool COMPACT>
 __global__ void __launch_bounds__(256) vsa_combine_bwd_kernel(const __nv_bfloat16* __restrict__ dO, BwdStrides3 ds,
                                                               const __nv_bfloat16* __restrict__ gate, BwdStrides3 gs,
                                                               const __nv_bfloat16* __restrict__ out_c,
@@ -31,7 +35,8 @@ __global__ void __launch_bounds__(256) vsa_combine_bwd_kernel(const __nv_bfloat1
   __shared__ float red[16][128];
   const int blk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int c8 = threadIdx.x & 15, rg = threadIdx.x >> 4;
-  const int len = block_len[blk];
+  const int len = COMPACT ? block_len[blk + 1] - block_len[blk] : block_len[blk];
+  const int row0 = COMPACT ? block_len[blk] : 0;
   const int64_t bh = int64_t(b) * H + h;
   float oc[8];
   {
@@ -50,7 +55,8 @@ __global__ void __launch_bounds__(256) vsa_combine_bwd_kernel(const __nv_bfloat1
 #pragma unroll
   for (int j = 0; j < VSA_TILE / 16; ++j) {
     const int r = rg + 16 * j;
-    const int64_t tok = int64_t(blk) * VSA_TILE + r;
+    if (COMPACT && r >= len) continue;
+    const int64_t tok = COMPACT ? int64_t(row0) + r : int64_t(blk) * VSA_TILE + r;
     const uint4 ud = *reinterpret_cast<const uint4*>(dO + b * ds.v[0] + tok * ds.v[1] + h * ds.v[2] + c8 * 8);
     const __nv_bfloat162* d2 = reinterpret_cast<const __nv_bfloat162*>(&ud);
     float dv[8];
@@ -223,10 +229,11 @@ __global__ void __launch_bounds__(256) softmax_rows_bwd_kernel(const __nv_bfloat
 }
 
 // dx[b, tok, h, :] = bf16(dx_s + d_mean[b, h, tile, :] / len[tile]) for tok % 64 < len[tile], else 0. One thread per 8
-// elements; dx may be dx_s (in place).
+// elements; dx may be dx_s (in place). COMPACT: block_len is block_off [nblk + 1], tile = row_block[tok], every row valid.
+template <bool COMPACT>
 __global__ void block_mean_bwd_kernel(const __nv_bfloat16* dx_s, BwdStrides3 ss, const __nv_bfloat16* __restrict__ d_mean,
                                       const int32_t* __restrict__ block_len, __nv_bfloat16* dx, BwdStrides3 os, int B, int S,
-                                      int H, int nblk) {
+                                      int H, int nblk, const int32_t* __restrict__ row_block) {
   const int64_t idx = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int64_t total = int64_t(B) * H * S * 16;
   if (idx >= total) return;
@@ -234,10 +241,10 @@ __global__ void block_mean_bwd_kernel(const __nv_bfloat16* dx_s, BwdStrides3 ss,
   const int tok = int((idx >> 4) % S);
   const int64_t bh = (idx >> 4) / S;
   const int h = int(bh % H), b = int(bh / H);
-  const int blk = tok / VSA_TILE;
-  const int len = __ldg(block_len + blk);
+  const int blk = COMPACT ? __ldg(row_block + tok) : tok / VSA_TILE;
+  const int len = COMPACT ? __ldg(block_len + blk + 1) - __ldg(block_len + blk) : __ldg(block_len + blk);
   uint4 o = make_uint4(0, 0, 0, 0);
-  if (tok - blk * VSA_TILE < len) {
+  if (COMPACT || tok - blk * VSA_TILE < len) {
     const uint4 us = *reinterpret_cast<const uint4*>(dx_s + b * ss.v[0] + int64_t(tok) * ss.v[1] + h * ss.v[2] + c8 * 8);
     const uint4 um = __ldg(reinterpret_cast<const uint4*>(d_mean + (bh * nblk + blk) * 128 + c8 * 8));
     const __nv_bfloat162* s2 = reinterpret_cast<const __nv_bfloat162*>(&us);
@@ -259,11 +266,15 @@ static bool strides_ok(const int64_t* s) { return s[0] % 8 == 0 && s[1] % 8 == 0
 
 using namespace fvb;
 
-extern "C" int fvb_vsa_combine_bwd(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides,
-                                   const void* out_c, const int32_t* block_len, int B, int S, int H, int nblk, void* d_gate,
-                                   const int64_t* dg_strides, void* d_out_c, void* d_out_c_t, int64_t ldt, void* stream) {
-  FVB_CHECK_ARG(dO && do_strides && out_c && block_len && d_out_c, "null pointer");
-  FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S == nblk * VSA_TILE, "S must be 64 * nblk (padded layout)");
+template <bool COMPACT>
+static int combine_bwd(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides, const void* out_c,
+                       const int32_t* block_tab, int B, int S, int H, int nblk, void* d_gate, const int64_t* dg_strides,
+                       void* d_out_c, void* d_out_c_t, int64_t ldt, void* stream) {
+  FVB_CHECK_ARG(dO && do_strides && out_c && block_tab && d_out_c, "null pointer");
+  if (COMPACT)
+    FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S > 0, "empty problem");
+  else
+    FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S == nblk * VSA_TILE, "S must be 64 * nblk (padded layout)");
   FVB_CHECK_ARG(gate == nullptr || g_strides != nullptr, "gate strides missing");
   FVB_CHECK_ARG(d_gate == nullptr || (gate != nullptr && dg_strides != nullptr), "d_gate needs gate and its strides");
   FVB_CHECK_ARG(d_out_c_t == nullptr || ldt >= nblk, "ldt too small");
@@ -275,12 +286,27 @@ extern "C" int fvb_vsa_combine_bwd(const void* dO, const int64_t* do_strides, co
     gs.v[i] = gate ? g_strides[i] : 0;
     dgs.v[i] = d_gate ? dg_strides[i] : 0;
   }
-  vsa_combine_bwd_kernel<<<dim3(nblk, H, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  vsa_combine_bwd_kernel<COMPACT><<<dim3(nblk, H, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(dO), ds, reinterpret_cast<const __nv_bfloat16*>(gate), gs,
-      reinterpret_cast<const __nv_bfloat16*>(out_c), block_len, reinterpret_cast<__nv_bfloat16*>(d_gate), dgs,
+      reinterpret_cast<const __nv_bfloat16*>(out_c), block_tab, reinterpret_cast<__nv_bfloat16*>(d_gate), dgs,
       reinterpret_cast<__nv_bfloat16*>(d_out_c), reinterpret_cast<__nv_bfloat16*>(d_out_c_t), ldt, nblk, H);
   FVB_CHECK_CUDA(cudaGetLastError());
   return FVB_OK;
+}
+
+extern "C" int fvb_vsa_combine_bwd(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides,
+                                   const void* out_c, const int32_t* block_len, int B, int S, int H, int nblk, void* d_gate,
+                                   const int64_t* dg_strides, void* d_out_c, void* d_out_c_t, int64_t ldt, void* stream) {
+  return combine_bwd<false>(dO, do_strides, gate, g_strides, out_c, block_len, B, S, H, nblk, d_gate, dg_strides, d_out_c,
+                            d_out_c_t, ldt, stream);
+}
+
+extern "C" int fvb_vsa_combine_bwd_compact(const void* dO, const int64_t* do_strides, const void* gate,
+                                           const int64_t* g_strides, const void* out_c, const int32_t* block_off, int B, int S,
+                                           int H, int nblk, void* d_gate, const int64_t* dg_strides, void* d_out_c,
+                                           void* d_out_c_t, int64_t ldt, void* stream) {
+  return combine_bwd<true>(dO, do_strides, gate, g_strides, out_c, block_off, B, S, H, nblk, d_gate, dg_strides, d_out_c,
+                           d_out_c_t, ldt, stream);
 }
 
 extern "C" int fvb_softmax_rows_bwd(const void* p, const void* dp, int64_t ld, int batch, int n, float scale, void* ds,
@@ -297,16 +323,31 @@ extern "C" int fvb_softmax_rows_bwd(const void* p, const void* dp, int64_t ld, i
   return FVB_OK;
 }
 
-extern "C" int fvb_block_mean_bwd(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_len,
-                                  int B, int H, int S, int nblk, void* dx, const int64_t* dx_strides, void* stream) {
-  FVB_CHECK_ARG(dx_s && s_strides && d_mean && block_len && dx && dx_strides, "null pointer");
-  FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S == nblk * VSA_TILE, "S must be 64 * nblk (padded layout)");
+template <bool COMPACT>
+static int mean_bwd(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_tab,
+                    const int32_t* row_block, int B, int H, int S, int nblk, void* dx, const int64_t* dx_strides, void* stream) {
+  FVB_CHECK_ARG(dx_s && s_strides && d_mean && block_tab && dx && dx_strides && (!COMPACT || row_block), "null pointer");
+  if (COMPACT)
+    FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S > 0, "empty problem");
+  else
+    FVB_CHECK_ARG(B > 0 && H > 0 && nblk > 0 && S == nblk * VSA_TILE, "S must be 64 * nblk (padded layout)");
   FVB_CHECK_ARG(strides_ok(s_strides) && strides_ok(dx_strides), "strides must be multiples of 8");
   const int64_t total = int64_t(B) * H * S * 16;
-  block_mean_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  block_mean_bwd_kernel<COMPACT><<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(dx_s), BwdStrides3{{s_strides[0], s_strides[1], s_strides[2]}},
-      reinterpret_cast<const __nv_bfloat16*>(d_mean), block_len, reinterpret_cast<__nv_bfloat16*>(dx),
-      BwdStrides3{{dx_strides[0], dx_strides[1], dx_strides[2]}}, B, S, H, nblk);
+      reinterpret_cast<const __nv_bfloat16*>(d_mean), block_tab, reinterpret_cast<__nv_bfloat16*>(dx),
+      BwdStrides3{{dx_strides[0], dx_strides[1], dx_strides[2]}}, B, S, H, nblk, row_block);
   FVB_CHECK_CUDA(cudaGetLastError());
   return FVB_OK;
+}
+
+extern "C" int fvb_block_mean_bwd(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_len,
+                                  int B, int H, int S, int nblk, void* dx, const int64_t* dx_strides, void* stream) {
+  return mean_bwd<false>(dx_s, s_strides, d_mean, block_len, nullptr, B, H, S, nblk, dx, dx_strides, stream);
+}
+
+extern "C" int fvb_block_mean_bwd_compact(const void* dx_s, const int64_t* s_strides, const void* d_mean,
+                                          const int32_t* block_off, const int32_t* row_block, int B, int H, int S, int nblk,
+                                          void* dx, const int64_t* dx_strides, void* stream) {
+  return mean_bwd<true>(dx_s, s_strides, d_mean, block_off, row_block, B, H, S, nblk, dx, dx_strides, stream);
 }

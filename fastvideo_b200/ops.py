@@ -633,6 +633,58 @@ def attention_blocklist_bwd(q, k, v, o, lse, dO, q2k_idx, q2k_num, k2q_idx, k2q_
     return dq, dk, dv
 
 
+def attention_sparse_bwd(q, k, v, o, lse, dO, q2k_idx, q2k_num, k2q_idx, k2q_num, q_off=None, q_len=None, kv_off=None,
+                         kv_len=None, softmax_scale=None, out=None):
+    """fvb_attention_sparse_bwd: backward of attention_blocklist in either layout, on the wgmma kernels. q/k/v/o/dO:
+    [B, S, H, 128] bf16 views (strided ok, as the forward takes them); lse fp32 [B, H, Sq] (unit stride along Sq) as
+    attention_blocklist(..., return_lse=True) returns it; q2k_idx int32 [B or 1, H or 1, nqb, capq] / q2k_num [.., nqb] and the
+    inverse k2q lists [.., nkb, capk] / [.., nkb]. q_off / q_len / kv_off / kv_len: the forward's tile tables (None: 64-row
+    tiles). Returns (dq, dk, dv) with q's / k's / v's shapes (BSHD); rows outside every tile (pad rows) are zero.
+    out = (dq, dk, dv) views to write into instead ((b, s, h) strides multiples of 8): only tile rows are written there."""
+    for n, t in (("q", q), ("k", k), ("v", v), ("o", o), ("dO", dO)):
+        _require_cuda_bf16(t, n)
+    B, Sq, H, d = q.shape
+    Skv = k.shape[1]
+    if softmax_scale is None:
+        softmax_scale = d ** -0.5
+    if (k.shape != (B, Skv, H, d) or v.shape != k.shape or o.shape != q.shape or dO.shape != q.shape
+            or lse.dtype != torch.float32 or lse.shape != (B, H, Sq) or lse.stride(2) != 1):
+        raise FvbError("attention_sparse_bwd: q/o/dO [B, Sq, H, 128], k/v [B, Skv, H, 128], lse fp32 [B, H, Sq]")
+    for t in (q2k_idx, q2k_num, k2q_idx, k2q_num):
+        if t.dtype != torch.int32 or not t.is_contiguous():
+            raise FvbError("attention_sparse_bwd: index lists must be contiguous int32")
+    ib, ih, nqb, capq = q2k_idx.shape
+    kb_, kh_, nkb, capk = k2q_idx.shape
+    for name, t, n in (("q_off", q_off, nqb + 1), ("q_len", q_len, nqb), ("kv_off", kv_off, nkb + 1), ("kv_len", kv_len, nkb)):
+        if t is not None:
+            _check_i32(t, name, n)
+    # without tile offsets, rows past a tile's length (pad rows) belong to no tile and are not written: zero them
+    if out is None:
+        alloc = lambda off, lens: torch.zeros if (off is None and lens is not None) else torch.empty
+        dq = alloc(q_off, q_len)((B, Sq, H, d), dtype=torch.bfloat16, device=q.device)
+        dk = alloc(kv_off, kv_len)((B, Skv, H, d), dtype=torch.bfloat16, device=q.device)
+        dv = alloc(kv_off, kv_len)((B, Skv, H, d), dtype=torch.bfloat16, device=q.device)
+    else:
+        dq, dk, dv = out
+        for n, t, want in (("dq", dq, q.shape), ("dk", dk, k.shape), ("dv", dv, k.shape)):
+            _require_cuda_bf16(t, n)
+            if t.shape != want:
+                raise FvbError(f"attention_sparse_bwd: {n} must have shape {tuple(want)}")
+    delta = torch.empty((B * H * Sq,), dtype=torch.float32, device=q.device)
+    sb = lambda nb, nh, n: (0 if nb == 1 else nh * n, 0 if nh == 1 else n)
+    isb, ish = sb(ib, ih, nqb)
+    ksb, ksh = sb(kb_, kh_, nkb)
+    check(lib().fvb_attention_sparse_bwd(ptr(q), ptr(k), ptr(v), ptr(o), ptr(dO), _f32p(lse), c_int64(lse.stride(0)),
+                                         c_int64(lse.stride(1)), ptr(dq), ptr(dk), ptr(dv), _f32p(delta), _bsh_strides(q),
+                                         _bsh_strides(k), _bsh_strides(v), _bsh_strides(o), _bsh_strides(dO), _bsh_strides(dq),
+                                         _bsh_strides(dk), _bsh_strides(dv), c_int(B), c_int(H), c_int(Sq), c_int(Skv), c_int(d),
+                                         c_float(softmax_scale), _i32p(q2k_idx), _i32p(q2k_num), c_int(capq), _i32p(k2q_idx),
+                                         _i32p(k2q_num), c_int(capk), c_int64(isb), c_int64(ish), c_int64(ksb), c_int64(ksh),
+                                         _i32p(q_off), _i32p(q_len), c_int(nqb), _i32p(kv_off), _i32p(kv_len), c_int(nkb),
+                                         stream_ptr()))
+    return dq, dk, dv
+
+
 def attention_bwd(q, k, v, o, lse, dO, softmax_scale=None):
     """fvb_attention_bwd: backward of the dense attention(). q/o/dO: [B, Sq, H, 128], k/v: [B, Skv, H, 128] bf16 views ((b, s, h)
     strides multiples of 8, as the forward takes them); lse fp32 [B, H, Sq] (unit stride along Sq), as attention(...,
@@ -839,31 +891,36 @@ def vsa_combine(out_s: torch.Tensor, out_c: torch.Tensor, gate: torch.Tensor | N
     return out
 
 
-# ---------------------------------------------------------------- VSA backward (padded layout: 64-row tiles)
+# ---------------------------------------------------------------- VSA backward (padded layout: 64-row tiles; or compact)
 def vsa_combine_bwd(dO: torch.Tensor, out_c: torch.Tensor, gate: torch.Tensor | None, block_len: torch.Tensor,
-                    d_gate: torch.Tensor | None = None):
+                    d_gate: torch.Tensor | None = None, block_off: torch.Tensor | None = None):
     """Backward of vsa_combine (fvb_vsa_combine_bwd). dO/gate/d_gate: [B, S, H, 128] views, S = 64 * nblk; out_c
     [B, H, nblk, 128] contiguous; block_len int32 [nblk]. d_gate (output, written when given) = dO * out_c on the valid
     rows and 0 on the pad rows (pad rows are not tokens: dO there counts as zero).
     Returns (d_out_c bf16 [B, H, nblk, 128], the same transposed [B, H, 128, nblk] as a view of a [.., ldt] buffer):
-    d_out_c = sum over each tile's valid rows of dO * gate (of dO without a gate), fp32 in a fixed order."""
+    d_out_c = sum over each tile's valid rows of dO * gate (of dO without a gate), fp32 in a fixed order.
+    block_off (int32 [nblk + 1]): the compact layout instead (fvb_vsa_combine_bwd_compact): tile i is rows
+    [block_off[i], block_off[i + 1]), every row a token; block_len is then not read."""
     for n, t in (("dO", dO), ("out_c", out_c), ("gate", gate), ("d_gate", d_gate)):
         if t is not None:
             _require_cuda_bf16(t, n)
     B, S, H, d = dO.shape
     nblk = out_c.shape[2]
-    if d != 128 or S != 64 * nblk or out_c.shape != (B, H, nblk, d) or not out_c.is_contiguous():
+    if d != 128 or (block_off is None and S != 64 * nblk) or out_c.shape != (B, H, nblk, d) or not out_c.is_contiguous():
         raise FvbError("dO must be [B, 64 * nblk, H, 128] and out_c contiguous [B, H, nblk, 128]")
     if d_gate is not None and gate is None:
         raise FvbError("d_gate needs the gate")
-    _check_i32(block_len, "block_len", nblk)
+    if block_off is None:
+        _check_i32(block_len, "block_len", nblk)
+    else:
+        _check_i32(block_off, "block_off", nblk + 1)
     d_out_c = torch.empty((B, H, nblk, d), dtype=torch.bfloat16, device=dO.device)
     ldt = (nblk + 7) // 8 * 8
     d_out_c_t = torch.empty((B, H, d, ldt), dtype=torch.bfloat16, device=dO.device)
-    check(lib().fvb_vsa_combine_bwd(ptr(dO), _bsh_strides(dO), ptr(gate), _bsh_strides(gate) if gate is not None else None,
-                                    ptr(out_c), _i32p(block_len), c_int(B), c_int(S), c_int(H), c_int(nblk), ptr(d_gate),
-                                    _bsh_strides(d_gate) if d_gate is not None else None, ptr(d_out_c), ptr(d_out_c_t),
-                                    c_int64(ldt), stream_ptr()))
+    fn = lib().fvb_vsa_combine_bwd if block_off is None else lib().fvb_vsa_combine_bwd_compact
+    check(fn(ptr(dO), _bsh_strides(dO), ptr(gate), _bsh_strides(gate) if gate is not None else None, ptr(out_c),
+             _i32p(block_len if block_off is None else block_off), c_int(B), c_int(S), c_int(H), c_int(nblk), ptr(d_gate),
+             _bsh_strides(d_gate) if d_gate is not None else None, ptr(d_out_c), ptr(d_out_c_t), c_int64(ldt), stream_ptr()))
     return d_out_c, d_out_c_t[..., :nblk]
 
 
@@ -890,22 +947,34 @@ def softmax_rows_bwd(p: torch.Tensor, dp: torch.Tensor, scale: float = 1.0, want
     return ds[..., :n]
 
 
-def block_mean_bwd(dx_s: torch.Tensor, d_mean: torch.Tensor, block_len: torch.Tensor, out: torch.Tensor | None = None):
+def block_mean_bwd(dx_s: torch.Tensor, d_mean: torch.Tensor, block_len: torch.Tensor, out: torch.Tensor | None = None,
+                   block_off: torch.Tensor | None = None, row_block: torch.Tensor | None = None):
     """Backward of block_mean in the padded layout added to dx_s (fvb_block_mean_bwd): dx = dx_s + d_mean / len on the valid
     rows of each 64-row tile, 0 on its pad rows. dx_s / out: [B, S, H, 128] views, S = 64 * nblk (out may be dx_s: in place);
-    d_mean [B, H, nblk, 128] contiguous; block_len int32 [nblk]."""
+    d_mean [B, H, nblk, 128] contiguous; block_len int32 [nblk].
+    block_off (int32 [nblk + 1]) with row_block (int32 [S]): the compact layout instead (fvb_block_mean_bwd_compact): every
+    row is a token of tile row_block[t], len = block_off[tile + 1] - block_off[tile]; block_len is then not read."""
     _require_cuda_bf16(dx_s, "dx_s")
     _require_cuda_bf16(d_mean, "d_mean")
     B, S, H, d = dx_s.shape
     nblk = d_mean.shape[2]
-    if d != 128 or S != 64 * nblk or d_mean.shape != (B, H, nblk, d) or not d_mean.is_contiguous():
+    if d != 128 or (block_off is None and S != 64 * nblk) or d_mean.shape != (B, H, nblk, d) or not d_mean.is_contiguous():
         raise FvbError("dx_s must be [B, 64 * nblk, H, 128] and d_mean contiguous [B, H, nblk, 128]")
-    _check_i32(block_len, "block_len", nblk)
+    if (block_off is None) != (row_block is None):
+        raise FvbError("the compact layout needs both block_off and row_block")
     if out is None:
         out = torch.empty((B, S, H, d), dtype=torch.bfloat16, device=dx_s.device)
     _require_cuda_bf16(out, "out")
-    check(lib().fvb_block_mean_bwd(ptr(dx_s), _bsh_strides(dx_s), ptr(d_mean), _i32p(block_len), c_int(B), c_int(H), c_int(S),
-                                   c_int(nblk), ptr(out), _bsh_strides(out), stream_ptr()))
+    if block_off is None:
+        _check_i32(block_len, "block_len", nblk)
+        check(lib().fvb_block_mean_bwd(ptr(dx_s), _bsh_strides(dx_s), ptr(d_mean), _i32p(block_len), c_int(B), c_int(H),
+                                       c_int(S), c_int(nblk), ptr(out), _bsh_strides(out), stream_ptr()))
+    else:
+        _check_i32(block_off, "block_off", nblk + 1)
+        _check_i32(row_block, "row_block", S)
+        check(lib().fvb_block_mean_bwd_compact(ptr(dx_s), _bsh_strides(dx_s), ptr(d_mean), _i32p(block_off), _i32p(row_block),
+                                               c_int(B), c_int(H), c_int(S), c_int(nblk), ptr(out), _bsh_strides(out),
+                                               stream_ptr()))
     return out
 
 

@@ -38,11 +38,12 @@ What install() registers, and the reference interface each piece stands behind:
                       to forward_cuda for the classes that got one.
   whole block         load_wan_block(): a reference WanTransformerBlock(_VSA)'s state_dict() -> wan_dit.WanBlock.
 
-Training: the dense backend (through B200AttentionImpl, backward fvb_attention_bwd), RMSNorm.forward_cuda (backward
-fvb_rmsnorm_bwd) and the fvb200_bf16 linear method (through linear_forward, backward fvb_linear_dgrad_bf16 /
-fvb_linear_wgrad_bf16 / fvb_bias_grad_bf16) are differentiable when grad is enabled and an input requires grad; without
-grad they run the same calls as before. The VSA impl above, the 8-bit backend and the FP8, INT8-weight and W8A8 linear
-methods are forward-only.
+Training: the dense backend (through B200AttentionImpl, backward fvb_attention_bwd), the VSA impl (through
+VideoSparseAttentionImpl: compact-layout backward on fvb_attention_sparse_bwd, fvb_vsa_combine_bwd_compact and
+fvb_block_mean_bwd_compact; tile / untile as autograd permutations), RMSNorm.forward_cuda (backward fvb_rmsnorm_bwd) and
+the fvb200_bf16 linear method (through linear_forward, backward fvb_linear_dgrad_bf16 / fvb_linear_wgrad_bf16 /
+fvb_bias_grad_bf16) are differentiable when grad is enabled and an input requires grad; without grad they run the same
+calls as before. The 8-bit backend and the FP8, INT8-weight and W8A8 linear methods are forward-only.
 
 There is no CPU fallback anywhere: with non-CUDA tensors these classes raise FvbError exactly like the rest of the
 package. uninstall() restores every patched attribute.
@@ -195,7 +196,10 @@ def _define():
 
     class Fvb200VideoSparseAttentionImpl(V.VideoSparseAttentionImpl):
         """preprocess_qkv -> forward(q, k, v, gate, md) -> postprocess_output, as DistributedAttention_VSA drives them
-        (attention/layer.py:172-245). "Tiling" is a permutation into compact tile-major order (no zero rows)."""
+        (attention/layer.py:172-245). "Tiling" is a permutation into compact tile-major order (no zero rows).
+        Differentiable (delegates to attention.VideoSparseAttentionImpl): with grad enabled and an input that requires
+        grad, tiling and untiling are autograd permutations and forward runs the compact-layout VSA backward; the forward
+        output is the same bits as without grad."""
 
         def __init__(self, num_heads: int, head_size: int, causal: bool = False, softmax_scale: float | None = None,
                      num_kv_heads: int | None = None, prefix: str = "", **extra_impl_args) -> None:

@@ -73,26 +73,38 @@ def video_sparse_attn_bshd(q, k, v, variable_block_sizes, topk: int, gate=None, 
 
 
 class _VideoSparseAttnFn(torch.autograd.Function):
-    """video_sparse_attn with autograd, padded layout. The forward runs the kernels of video_sparse_attn_bshd's block-list
-    path in the same order, so its output is bit-identical, and keeps what the backward needs. The backward is what torch
-    autograd computes for the reference composite (ops.py:65-133); the top-k selection has no gradient:
-      sparse branch   fvb_attention_blocklist_bwd (kv -> q lists from the transposed block map)
-      combine         fvb_vsa_combine_bwd: d_gate = dO * out_c, d_out_c = per-tile sum of dO * gate
+    """video_sparse_attn with autograd, in either token layout. The forward runs the kernels of video_sparse_attn_bshd's
+    block-list path in the same order, so its output is bit-identical, and keeps what the backward needs. The backward is
+    what torch autograd computes for the reference composite (ops.py:65-133); the top-k selection has no gradient:
+      sparse branch   padded: fvb_attention_blocklist_bwd; compact: fvb_attention_sparse_bwd (kv -> q lists from the
+                      transposed block map)
+      combine         fvb_vsa_combine_bwd(_compact): d_gate = dO * out_c, d_out_c = per-tile sum of dO * gate
       compression     d_attn = d_out_c v_c^T, d_v_c = attn^T d_out_c, d_scores' = softmax backward / sqrt(d),
                       d_q_c = d_scores' k_c, d_k_c = d_scores'^T q_c (fvb_gemm_batched_bf16; the transposed operands
                       come from the kernels that produce them)
-      block means     fvb_block_mean_bwd: dq = dq_s + d_q_c / len on the valid rows, 0 on the pad rows (k, v likewise)
+      block means     fvb_block_mean_bwd(_compact): dq = dq_s + d_q_c / len on the token rows, 0 on pad rows (k, v likewise)
+    Padded layout (block_off None): q, k, v, gate are [B, H, S_pad, 128] (the reference signature). Compact layout: they are
+    [B, S, H, 128] views in tile-major order, block_off int32 [nblk + 1] / row_block int32 [S] the tile tables.
     block_map (bool [B, H, nblk, nblk], or None for the top-k of the block scores) fixes the selection; it is how the
     tests reach q blocks without keys, which top-k never produces."""
 
     @staticmethod
-    def forward(ctx, q, k, v, gate, vbs, topk, block_map):
-        B, H, S, d = q.shape
-        nblk = S // 64
-        qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
-        q_c, q_ct = ops.block_mean(qt, nblk, None, vbs, want_transposed=True)
-        k_c, k_ct = ops.block_mean(kt, nblk, None, vbs, want_transposed=True)
-        v_c, v_ct = ops.block_mean(vt, nblk, None, vbs, want_transposed=True)
+    def forward(ctx, q, k, v, gate, vbs, topk, block_map, block_off=None, row_block=None):
+        if SPARSE_KERNEL != "ws":
+            raise ops.FvbError("the VSA backward needs the block-list sparse kernel (FVB_VSA_KERNEL=ws)")
+        compact = block_off is not None
+        if compact:
+            B, S, H, d = q.shape
+            nblk = vbs.numel()
+            qt, kt, vt, gt = q, k, v, gate
+        else:
+            B, H, S, d = q.shape
+            nblk = S // 64
+            qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
+            gt = None if gate is None else gate.transpose(1, 2)
+        q_c, q_ct = ops.block_mean(qt, nblk, block_off, vbs, want_transposed=True)
+        k_c, k_ct = ops.block_mean(kt, nblk, block_off, vbs, want_transposed=True)
+        v_c, v_ct = ops.block_mean(vt, nblk, block_off, vbs, want_transposed=True)
         scores = ops.gemm_batched(q_c.view(B * H, nblk, d), k_c.view(B * H, nblk, d), div=math.sqrt(d))
         attn = ops.softmax_rows(scores)
         out_c = ops.gemm_batched(attn, v_ct.reshape(B * H, d, -1)).contiguous().view(B, H, nblk, d)
@@ -101,26 +113,40 @@ class _VideoSparseAttnFn(torch.autograd.Function):
         else:
             q2k_idx, q2k_num = ops.map_to_index(block_map.contiguous())
         q2k_idx, q2k_num = q2k_idx.view(B, H, nblk, nblk), q2k_num.view(B, H, nblk)
-        out_s, lse = ops.attention_blocklist(qt, kt, vt, q2k_idx, q2k_num, softmax_scale=d ** -0.5, q_len=vbs, kv_len=vbs,
-                                             nkb=nblk, return_lse=True)
-        out = torch.empty_like(q)
-        ops.vsa_combine(out_s, out_c, None if gate is None else gate.transpose(1, 2), out=out.transpose(1, 2))
+        out_s, lse = ops.attention_blocklist(qt, kt, vt, q2k_idx, q2k_num, softmax_scale=d ** -0.5, q_off=block_off,
+                                             kv_off=block_off, q_len=vbs, kv_len=vbs, nkb=nblk, return_lse=True)
+        if compact:
+            out = ops.vsa_combine(out_s, out_c, gt, row_block=row_block)
+        else:
+            out = torch.empty_like(q)
+            ops.vsa_combine(out_s, out_c, gt, out=out.transpose(1, 2))
         ctx.save_for_backward(q, k, v, gate, vbs, q_ct, k_ct, v_c, attn, out_c, out_s, lse, q2k_idx, q2k_num,
-                              block_map.view(B, H, nblk, nblk))
+                              block_map.view(B, H, nblk, nblk), block_off, row_block)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        q, k, v, gate, vbs, q_ct, k_ct, v_c, attn, out_c, out_s, lse, q2k_idx, q2k_num, block_map = ctx.saved_tensors
-        B, H, S, d = q.shape
-        nblk = S // 64
-        BH = B * H
-        go = grad_out.to(torch.bfloat16).contiguous().transpose(1, 2)
-        qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
+        (q, k, v, gate, vbs, q_ct, k_ct, v_c, attn, out_c, out_s, lse, q2k_idx, q2k_num, block_map, block_off,
+         row_block) = ctx.saved_tensors
+        compact = block_off is not None
         want_d_gate = gate is not None and ctx.needs_input_grad[3]
-        d_gate = torch.empty_like(gate) if want_d_gate else None
-        d_out_c, d_out_c_t = ops.vsa_combine_bwd(go, out_c, None if gate is None else gate.transpose(1, 2), vbs,
-                                                 d_gate=None if d_gate is None else d_gate.transpose(1, 2))
+        if compact:
+            B, S, H, d = q.shape
+            nblk = vbs.numel()
+            go = grad_out.to(torch.bfloat16).contiguous()
+            qt, kt, vt, gt = q, k, v, gate
+            d_gate = torch.empty((B, S, H, d), dtype=torch.bfloat16, device=q.device) if want_d_gate else None
+            dgt = d_gate
+        else:
+            B, H, S, d = q.shape
+            nblk = S // 64
+            go = grad_out.to(torch.bfloat16).contiguous().transpose(1, 2)
+            qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
+            gt = None if gate is None else gate.transpose(1, 2)
+            d_gate = torch.empty_like(gate) if want_d_gate else None
+            dgt = None if d_gate is None else d_gate.transpose(1, 2)
+        BH = B * H
+        d_out_c, d_out_c_t = ops.vsa_combine_bwd(go, out_c, gt, vbs, d_gate=dgt, block_off=block_off)
         # compression branch
         d_attn = ops.gemm_batched(d_out_c.view(BH, nblk, d), v_c.view(BH, nblk, d))
         d_scores, d_scores_t, attn_t = ops.softmax_rows_bwd(attn, d_attn, scale=d ** -0.5, want_transposed=True)
@@ -129,10 +155,16 @@ class _VideoSparseAttnFn(torch.autograd.Function):
         d_k_c = ops.gemm_batched(d_scores_t, q_ct.reshape(BH, d, nblk))
         # sparse branch: kv block -> the q blocks that selected it, from the transposed block map
         k2q_idx, k2q_num = ops.map_to_index(block_map.transpose(-1, -2).contiguous())
-        dq, dk, dv = ops.attention_blocklist_bwd(qt, kt, vt, out_s, lse, go, q2k_idx, q2k_num, k2q_idx, k2q_num, kv_len=vbs)
+        if compact:
+            dq, dk, dv = ops.attention_sparse_bwd(qt, kt, vt, out_s, lse, go, q2k_idx, q2k_num, k2q_idx, k2q_num,
+                                                  q_off=block_off, q_len=vbs, kv_off=block_off, kv_len=vbs)
+        else:
+            dq, dk, dv = ops.attention_blocklist_bwd(qt, kt, vt, out_s, lse, go, q2k_idx, q2k_num, k2q_idx, k2q_num, kv_len=vbs)
         for dx, dc in ((dq, d_q_c), (dk, d_k_c), (dv, d_v_c)):
-            ops.block_mean_bwd(dx, dc.contiguous().view(B, H, nblk, d), vbs, out=dx)
-        return dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2), d_gate, None, None, None
+            ops.block_mean_bwd(dx, dc.contiguous().view(B, H, nblk, d), vbs, out=dx, block_off=block_off, row_block=row_block)
+        if compact:
+            return dq, dk, dv, d_gate, None, None, None, None, None
+        return dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2), d_gate, None, None, None, None, None
 
 
 def video_sparse_attn(q, k, v, variable_block_sizes, q_variable_block_sizes, topk, block_size=64,
@@ -148,8 +180,6 @@ def video_sparse_attn(q, k, v, variable_block_sizes, q_variable_block_sizes, top
         raise ValueError("q_seq_len and kv_seq_len must be divisible by block_elements=64")
     inputs = (q, k, v) if compress_attn_weight is None else (q, k, v, compress_attn_weight)
     if torch.is_grad_enabled() and any(t.requires_grad for t in inputs):
-        if SPARSE_KERNEL != "ws":
-            raise ops.FvbError("the VSA backward needs the block-list sparse kernel (FVB_VSA_KERNEL=ws)")
         vbs = variable_block_sizes.to(torch.int32).contiguous()
         return _VideoSparseAttnFn.apply(q, k, v, compress_attn_weight, vbs, topk, None)
     gate = None if compress_attn_weight is None else compress_attn_weight.transpose(1, 2)

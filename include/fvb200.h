@@ -379,6 +379,32 @@ int fvb_attention_bwd(const void* q, const void* k, const void* v, const void* o
                       const int64_t* dv_strides, int B, int H, int Sq, int Skv, int head_dim, float softmax_scale,
                       void* stream);
 
+/* Backward of fvb_attention_blocklist_fwd in either layout, on the wgmma kernels of fvb_attention_bwd. Arguments as in
+ * fvb_attention_blocklist_bwd, plus the forward's lse strides (lse[b * lse_stride_b + h * lse_stride_h + s]) and its tile
+ * addressing: q tile i starts at row q_off[i] (q_off NULL: 64 i) and has q_len[i] valid rows (q_len NULL: q_off[i + 1] -
+ * q_off[i], else 64), at most 64 and never past Sq; kv tiles likewise from kv_off / kv_len / Skv. nqb / nkb tiles; q2k lists
+ * [.., nqb, capq] of kv tiles, k2q lists [.., nkb, capk] of q tiles, both ascending (k2q = the transposed block map's lists).
+ * Per (b, h), for the pairs (q tile, kv tile) the lists select, over valid q rows i and valid keys j, fp32 accumulation:
+ *   delta_i = sum_c dO[i, c] * O[i, c]
+ *   P_ij = exp2(q_i . k_j * softmax_scale * log2 e - lse_i)   (ex2.approx)
+ *   dP_ij = dO_i . v_j         dS_ij = P_ij * (dP_ij - delta_i) * softmax_scale
+ *   dV_j = sum_i bf16(P_ij) dO_i      dK_j = sum_i bf16(dS_ij) q_i      dQ_i = sum_j bf16(dS_ij) k_j
+ * Tail rules: a kv tile's keys at or past its valid length give P = 0; q rows at or past a q tile's valid length take no
+ * part (lse = +inf, delta = 0 for them), so the next tile's rows that a 64-row box starting at off[i] also reads count for
+ * nothing. Only the valid rows of each tile are stored: rows outside every tile (pad rows of the padded layout) are not
+ * written, and a tile never writes another tile's rows. A tile whose list is empty gets zeros. The arithmetic of
+ * fvb_attention_bwd; deterministic (one CTA owns two 64-row tiles and walks the union of their lists; no float atomics). */
+int fvb_attention_sparse_bwd(const void* q, const void* k, const void* v, const void* o, const void* dO, const float* lse,
+                             int64_t lse_stride_b, int64_t lse_stride_h, void* dq, void* dk, void* dv, float* delta_ws,
+                             const int64_t* q_strides, const int64_t* k_strides, const int64_t* v_strides,
+                             const int64_t* o_strides, const int64_t* do_strides, const int64_t* dq_strides,
+                             const int64_t* dk_strides, const int64_t* dv_strides, int B, int H, int Sq, int Skv, int head_dim,
+                             float softmax_scale, const int32_t* q2k_idx, const int32_t* q2k_num, int capq,
+                             const int32_t* k2q_idx, const int32_t* k2q_num, int capk, int64_t idx_stride_b,
+                             int64_t idx_stride_h, int64_t kidx_stride_b, int64_t kidx_stride_h, const int32_t* q_off,
+                             const int32_t* q_len, int nqb, const int32_t* kv_off, const int32_t* kv_len, int nkb,
+                             void* stream);
+
 /* --------------------------------------------------------------------------------------------
  * Index / mask construction (integer, bit-exact with the reference)
  * -------------------------------------------------------------------------------------------- */
@@ -463,14 +489,14 @@ int fvb_gather_rows(const void* in, int64_t in_batch_stride, int64_t in_ld, cons
                     int64_t out_batch_stride, int64_t out_ld, int64_t n_out, int width, int B, void* stream);
 
 /* --------------------------------------------------------------------------------------------
- * Video Sparse Attention backward, padded layout only: S = 64 * nblk token rows, tile i = rows [64 i, 64 i + 64) of which
+ * Video Sparse Attention backward. Padded layout: S = 64 * nblk token rows, tile i = rows [64 i, 64 i + 64) of which
  * the first len[i] = block_len[i] (variable_block_sizes) are valid. The backward of video_sparse_attn
  * (fastvideo-kernel/python/fastvideo_kernel/ops.py:65-133) as torch autograd differentiates it, top-k selection excluded:
  *   combine:      fvb_vsa_combine_bwd
  *   compression:  d_attn = d_out_c v_c^T,  d_v_c = attn^T d_out_c  (fvb_gemm_batched_bf16),
  *                 d_scores' = fvb_softmax_rows_bwd(attn, d_attn, scale = 1 / sqrt(d)),
  *                 d_q_c = d_scores' k_c,  d_k_c = d_scores'^T q_c  (fvb_gemm_batched_bf16)
- *   sparse:       dq_s, dk_s, dv_s = fvb_attention_blocklist_bwd
+ *   sparse:       dq_s, dk_s, dv_s = fvb_attention_blocklist_bwd (compact layout: fvb_attention_sparse_bwd)
  *   block means:  fvb_block_mean_bwd (dq from dq_s and d_q_c, dk and dv likewise)
  *
  * Pad rows are not tokens: every gradient below treats dO there as zero (the forward's sparse-branch rows there are zero,
@@ -496,6 +522,15 @@ int fvb_gather_rows(const void* in, int64_t in_batch_stride, int64_t in_ld, cons
  *   dx[t, c] = 0                                                        for the pad rows
  *   dx_s, dx [B, S, H, 128] through (b, s, h) element strides (multiples of 8); dx may be dx_s (in place). d_mean bf16
  *   [B, H, nblk, 128] contiguous.
+ *
+ * Compact layout (the *_compact variants): S token rows in tile-major order without pad rows, tile i = rows
+ *   [block_off[i], block_off[i + 1]) (block_off int32 [nblk + 1], as fvb_block_mean takes it), row_block int32 [S] = the tile
+ *   of each row (as fvb_vsa_combine takes it). Every row is a token, so there are no pad-row zeroes:
+ *   fvb_vsa_combine_bwd_compact: d_gate[t, c] = bf16(dO[t, c] * out_c[tile(t), c]) for every row; d_out_c[i, c] = the sum
+ *     over rows block_off[i] + r, r < block_off[i + 1] - block_off[i], in the fixed order of fvb_vsa_combine_bwd (row r in
+ *     group r % 16). Other arguments as there.
+ *   fvb_block_mean_bwd_compact: dx[t, c] = bf16(dx_s[t, c] + d_mean[tile(t), c] / len) for every row t, tile(t) =
+ *     row_block[t], len = block_off[tile + 1] - block_off[tile]. Other arguments as in fvb_block_mean_bwd.
  * -------------------------------------------------------------------------------------------- */
 int fvb_vsa_combine_bwd(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides,
                         const void* out_c, const int32_t* block_len, int B, int S, int H, int nblk, void* d_gate,
@@ -506,6 +541,14 @@ int fvb_softmax_rows_bwd(const void* p, const void* dp, int64_t ld, int batch, i
 
 int fvb_block_mean_bwd(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_len, int B,
                        int H, int S, int nblk, void* dx, const int64_t* dx_strides, void* stream);
+
+int fvb_vsa_combine_bwd_compact(const void* dO, const int64_t* do_strides, const void* gate, const int64_t* g_strides,
+                                const void* out_c, const int32_t* block_off, int B, int S, int H, int nblk, void* d_gate,
+                                const int64_t* dg_strides, void* d_out_c, void* d_out_c_t, int64_t ldt, void* stream);
+
+int fvb_block_mean_bwd_compact(const void* dx_s, const int64_t* s_strides, const void* d_mean, const int32_t* block_off,
+                               const int32_t* row_block, int B, int H, int S, int nblk, void* dx, const int64_t* dx_strides,
+                               void* stream);
 
 /* --------------------------------------------------------------------------------------------
  * Wan VAE decode (channels-last frames x[t][h][w][c], bf16)

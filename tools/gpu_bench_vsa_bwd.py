@@ -6,7 +6,11 @@ the 21 x 45 x 80 latent grid in 4 x 4 x 4 tiles (1440 tiles, S_pad = 92 160), 40
     combine (fvb_vsa_combine_bwd), block means (three fvb_block_mean_bwd);
   * the sparse backward's rate on the model 2.5 x forward FLOPs, forward = 4 * 64 * 64 * 128 per selected (q block, kv
     block) pair, against the H100 SXM data-sheet 989 TFLOP/s (bf16 dense, 700 W);
-  * the row kernels' bytes moved (each tensor read or written once) per second, against 3.35 TB/s.
+  * the row kernels' bytes moved (each tensor read or written once) per second, against 3.35 TB/s;
+  * the compact layout (tile-major, no pad rows, S = 75 600) through VideoSparseAttentionImpl.forward: forward without
+    grad, forward with grad, forward + backward, and its sparse stage alone (inverse lists + fvb_attention_sparse_bwd);
+  * on the padded layout's lists, fvb_attention_sparse_bwd (wgmma) and fvb_attention_blocklist_bwd (mma.sync) alternating
+    in one run, each with its rate on the same FLOP model.
 The card's name, power limit and max SM clock are read in the same run. Writes <out>/bench_vsa_bwd.json.
 Usage: python tools/gpu_bench_vsa_bwd.py [--iters N] [--out DIR]"""
 import argparse
@@ -87,7 +91,7 @@ def main():
 
     # the backward's stages on one forward's saved tensors (the calls of _VideoSparseAttnFn.backward)
     (q_, k_, v_, gate_, vbs_, q_ct, k_ct, v_c, attn, out_c, out_s, lse, q2k_idx, q2k_num,
-     block_map) = out_g.grad_fn.saved_tensors
+     block_map) = out_g.grad_fn.saved_tensors[:15]
     BH = B * H
     go = dO.contiguous().transpose(1, 2)
     qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
@@ -134,6 +138,70 @@ def main():
               "softmax_rows_bwd_alone": 5 * sq}  # p, dp in; ds, ds^T, p^T out
     res["row_kernels"] = {n: {"bytes": b, "ms": st[n], "TB_s": b / (st[n] * 1e-3) / 1e12,
                               "share_of_3.35_TB_s": b / (st[n] * 1e-3) / 1e12 / HBM_TBS} for n, b in nbytes.items()}
+
+    # ---- compact layout, the plug-in's VSA impl
+    from types import SimpleNamespace
+    from fastvideo_b200.attention import VideoSparseAttentionImpl
+    off = torch.zeros(nblk + 1, dtype=torch.int32, device="cuda")
+    off[1:] = torch.cumsum(vbs, 0)
+    row_block = torch.repeat_interleave(torch.arange(nblk, device="cuda", dtype=torch.int32), vbs.long())
+    md = SimpleNamespace(VSA_sparsity=1.0 - (TOPK - 0.5) / nblk, variable_block_sizes=vbs, block_offsets=off,
+                         row_block=row_block)
+    comp = [t[:, :, valid].transpose(1, 2).contiguous() for t in (q, k, v, gate, dO)]
+    res["S_compact"] = comp[0].shape[1]
+    cleaves = [t.clone().requires_grad_(True) for t in comp[:4]]
+    impl = VideoSparseAttentionImpl(HEADS, d)
+
+    def c_nograd():
+        with torch.no_grad():
+            return impl.forward(*comp[:4], md)
+
+    def c_grad():
+        return impl.forward(*cleaves, md)
+
+    def c_fwd_bwd():
+        for t in cleaves:
+            t.grad = None
+        c_grad().backward(comp[4])
+
+    c_out = c_grad()
+    res["compact_forward_bit_identical_with_grad"] = bool(torch.equal(c_nograd(), c_out.detach()))
+    res["compact_forward_ms"] = time_ms(c_nograd, args.iters)
+    res["compact_forward_with_grad_ms"] = time_ms(c_grad, args.iters)
+    res["compact_forward_backward_ms"] = time_ms(c_fwd_bwd, args.iters)
+    sv = c_out.grad_fn.saved_tensors
+    c_q2k_idx, c_q2k_num, c_map = sv[12], sv[13], sv[14]
+    c_go = comp[4]
+
+    def c_sparse():
+        k2q_idx, k2q_num = ops.map_to_index(c_map.transpose(-1, -2).contiguous())
+        ops.attention_sparse_bwd(*comp[:3], sv[10], sv[11], c_go, c_q2k_idx, c_q2k_num, k2q_idx, k2q_num, q_off=off,
+                                 q_len=vbs, kv_off=off, kv_len=vbs)
+
+    res["compact_sparse_stage_ms"] = time_ms(c_sparse, args.iters)
+    c_pairs = int(c_q2k_num.long().sum())
+    res["compact_sparse_bwd_tflops_at_2.5x_fwd"] = 2.5 * 4.0 * c_pairs * 64 * 64 * d / (res["compact_sparse_stage_ms"] * 1e-3) / 1e12
+
+    # ---- the two sparse backward kernels on the padded layout's lists, alternating
+    k2q = ops.map_to_index(block_map.transpose(-1, -2).contiguous())
+    kern = {"fvb_attention_sparse_bwd": lambda: ops.attention_sparse_bwd(qt, kt, vt, out_s, lse, go, q2k_idx, q2k_num, *k2q,
+                                                                         q_len=vbs, kv_len=vbs),
+            "fvb_attention_blocklist_bwd": lambda: ops.attention_blocklist_bwd(qt, kt, vt, out_s, lse, go, q2k_idx, q2k_num,
+                                                                               *k2q, kv_len=vbs)}
+    ms = {n: [] for n in kern}
+    for _ in range(3):
+        for n, fn in kern.items():
+            ms[n].append(time_ms(fn, args.iters))
+    res["padded_lists_kernel_ms"] = {n: min(v) for n, v in ms.items()}
+    res["padded_lists_kernel_ms_all"] = ms
+    res["padded_lists_kernel_tflops_at_2.5x_fwd"] = {n: 2.5 * fwd_flop / (t * 1e-3) / 1e12
+                                                    for n, t in res["padded_lists_kernel_ms"].items()}
+    res["sparse_bwd_speedup_over_mma_sync"] = (res["padded_lists_kernel_ms"]["fvb_attention_blocklist_bwd"]
+                                               / res["padded_lists_kernel_ms"]["fvb_attention_sparse_bwd"])
+    a, b = kern["fvb_attention_sparse_bwd"](), kern["fvb_attention_blocklist_bwd"]()
+    m = valid.view(1, -1, 1, 1)
+    res["padded_lists_rel_l2_new_vs_mma_sync"] = {n: float(((x.float() - y.float()) * m).norm() / ((y.float() * m).norm() + 1e-30))
+                                                   for n, x, y in zip(("dq", "dk", "dv"), a, b)}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "bench_vsa_bwd.json"), "w") as f:
         json.dump(res, f, indent=1)
