@@ -32,6 +32,9 @@ def lib() -> ctypes.CDLL:
         _lib.fvb_attention_8bit_workspace_bytes.restype = c_int64
         _lib.fvb_rmsnorm_bwd_workspace_bytes.restype = c_int64
         _lib.fvb_bias_grad_bf16_workspace_bytes.restype = c_int64
+        _lib.fvb_resid_gate_bwd_workspace_bytes.restype = c_int64
+        _lib.fvb_layernorm_modulate_bwd_workspace_bytes.restype = c_int64
+        _lib.fvb_rmsnorm_rope_bwd_workspace_bytes.restype = c_int64
     return _lib
 
 

@@ -32,7 +32,7 @@ import torch
 from . import ops
 from .distributed import out_proj_sp
 from .rope import get_rotary_pos_embed
-from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail
+from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail, refuse_grad
 
 GLOBAL_ATTN_COMPAT_MAX_LATENT_FRAMES = 21  # causal_wanvideo.py:32
 
@@ -205,6 +205,7 @@ def causal_block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb
     rel = ccfg.rope_cache_policy == "relativistic"
     S, D = x.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
+    refuse_grad("the causal block (per-frame bf16 modulation)", blk, x, ctx, temb)
     tpf = S // temb.shape[0]
     fs = tpf if frame_seqlen is None else int(frame_seqlen)
     mod = Modulation.per_frame(blk, temb, tpf)
@@ -407,6 +408,7 @@ class SPCausalWanDiT:
         cfg, ccfg = m.cfg, m.ccfg
         D, d = cfg.hidden_size, cfg.head_dim
         fs, S, n = st["fs"], st["S"], st["n"]
+        refuse_grad("the sequence-parallel causal block", blk, x, ctx, temb)
         mod = Modulation.per_frame(blk, temb, n)
         n1 = mod.norm1(x, cfg.eps)
         segs, (k0, k1) = cache.advance(current_start, S, ccfg.local_attn_size, fs)

@@ -663,11 +663,16 @@ FVB_DEVICE float2 block_sum2(float2 v, float2* red) {
   return t;
 }
 
-__global__ void __launch_bounds__(EW_THREADS) rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx,
-                                                                 const __nv_bfloat16* __restrict__ w,
-                                                                 const __nv_bfloat16* __restrict__ dy, int64_t lddy,
-                                                                 __nv_bfloat16* __restrict__ dx, int64_t lddx,
-                                                                 float* __restrict__ dw_part, int M, int D, float eps) {
+// ROPE (fvb_rmsnorm_rope_bwd): dy is the gradient of the rotated output; each row is first un-rotated with the forward's
+// table row, dn = bf16(R^T dy) per interleaved pair, and dn takes dy's place below.
+template <bool ROPE>
+FVB_DEVICE void rmsnorm_bwd_body(const __nv_bfloat16* __restrict__ x, int64_t ldx,
+                                                 const __nv_bfloat16* __restrict__ w,
+                                                 const __nv_bfloat16* __restrict__ dy, int64_t lddy,
+                                                 __nv_bfloat16* __restrict__ dx, int64_t lddx,
+                                                 float* __restrict__ dw_part, int M, int D, float eps,
+                                                 const float* __restrict__ cos_t, const float* __restrict__ sin_t,
+                                                 const int32_t* __restrict__ rope_row, int head_dim) {
   __shared__ float2 red[32];
   const int nchunks = D >> 3;
   float acc[EW_MAX_CHUNKS][8];
@@ -684,6 +689,19 @@ __global__ void __launch_bounds__(EW_THREADS) rmsnorm_bwd_kernel(const __nv_bflo
       if (ch < nchunks) {
         unpack8(*reinterpret_cast<const uint4*>(x + row * ldx + (ch << 3)), xv[c]);
         unpack8(*reinterpret_cast<const uint4*>(dy + row * lddy + (ch << 3)), dv[c]);
+        if constexpr (ROPE) {
+          // forward: o[2i] = n[2i] c[2i] - n[2i+1] s[2i], o[2i+1] = n[2i+1] c[2i+1] + n[2i] s[2i+1]
+          const int64_t prow = rope_row != nullptr ? int64_t(rope_row[row]) : row;
+          float cs[8], sn[8];
+          load8_f32(cos_t + prow * head_dim + (ch << 3) % head_dim, cs);
+          load8_f32(sin_t + prow * head_dim + (ch << 3) % head_dim, sn);
+#pragma unroll
+          for (int i = 0; i < 8; i += 2) {
+            const float g0 = dv[c][i], g1 = dv[c][i + 1];
+            dv[c][i] = bf16_round(__fadd_rn(__fmul_rn(g0, cs[i]), __fmul_rn(g1, sn[i + 1])));
+            dv[c][i + 1] = bf16_round(__fsub_rn(__fmul_rn(g1, cs[i + 1]), __fmul_rn(g0, sn[i])));
+          }
+        }
         float wv[8];
         if (w != nullptr) unpack8(__ldg(reinterpret_cast<const uint4*>(w) + ch), wv);
 #pragma unroll
@@ -724,6 +742,36 @@ __global__ void __launch_bounds__(EW_THREADS) rmsnorm_bwd_kernel(const __nv_bflo
       dst[1] = make_float4(acc[c][4], acc[c][5], acc[c][6], acc[c][7]);
     }
   }
+}
+
+__global__ void __launch_bounds__(EW_THREADS) rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx,
+                                                                 const __nv_bfloat16* __restrict__ w,
+                                                                 const __nv_bfloat16* __restrict__ dy, int64_t lddy,
+                                                                 __nv_bfloat16* __restrict__ dx, int64_t lddx,
+                                                                 float* __restrict__ dw_part, int M, int D, float eps) {
+  rmsnorm_bwd_body<false>(x, ldx, w, dy, lddy, dx, lddx, dw_part, M, D, eps, nullptr, nullptr, nullptr, 0);
+}
+
+// Up to two tensors (q and k) per launch, blockIdx.y selects; tensor t's dw partials go to dw_part + t * gridDim.x * D.
+struct RmsRopeBwdArgs {
+  const __nv_bfloat16* x[2];
+  const __nv_bfloat16* w[2];
+  const __nv_bfloat16* dy[2];
+  __nv_bfloat16* dx[2];
+  int64_t ldx[2], lddy[2], lddx[2];
+};
+
+__global__ void __launch_bounds__(EW_THREADS) rmsnorm_rope_bwd_kernel(RmsRopeBwdArgs a, float* __restrict__ dw_part,
+                                                                      const float* __restrict__ cos_t,
+                                                                      const float* __restrict__ sin_t,
+                                                                      const int32_t* __restrict__ rope_row, int M, int D,
+                                                                      int head_dim, float eps) {
+  // fields selected with ternaries, not indexed by blockIdx.y: a dynamic index would copy the arrays to local memory
+  const bool t = blockIdx.y != 0;
+  rmsnorm_bwd_body<true>(t ? a.x[1] : a.x[0], t ? a.ldx[1] : a.ldx[0], t ? a.w[1] : a.w[0], t ? a.dy[1] : a.dy[0],
+                         t ? a.lddy[1] : a.lddy[0], t ? a.dx[1] : a.dx[0], t ? a.lddx[1] : a.lddx[0],
+                         dw_part != nullptr ? dw_part + int64_t(blockIdx.y) * gridDim.x * D : nullptr, M, D, eps, cos_t,
+                         sin_t, rope_row, head_dim);
 }
 
 __global__ void __launch_bounds__(256) rmsnorm_bwd_dw_kernel(const float* __restrict__ dw_part, int nparts, int D,
@@ -777,6 +825,170 @@ __global__ void __launch_bounds__(BG_THREADS) bias_grad_kernel(const __nv_bfloat
   float4* dst = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * N + col);
   dst[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
   dst[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// fp32 column sums of per-part partials, added in part order (the fp32 twin of rmsnorm_bwd_dw_kernel)
+__global__ void __launch_bounds__(256) colsum_f32_kernel(const float* __restrict__ part, int nparts, int N, float* __restrict__ out) {
+  const int col = blockIdx.x * 256 + threadIdx.x;
+  if (col >= N) return;
+  float s = 0.f;
+  for (int i = 0; i < nparts; ++i) s = __fadd_rn(s, __ldg(part + int64_t(i) * N + col));
+  out[col] = s;
+}
+
+// ------------------------------------------------------------------------------------------
+// Gated-residual backward (fvb_resid_gate_bwd; arithmetic in include/fvb200.h). The layout of bias_grad_kernel: blockIdx.y
+// picks 1024 columns (8 per thread), blockIdx.x one of BG_PARTS fixed row sets; the fp32 partials of sum dout * y (d_gate)
+// and of sum dy (bias grad) go to part[0][part][N] and part[1][part][N].
+// ------------------------------------------------------------------------------------------
+template <bool DOUT_F32>
+__global__ void __launch_bounds__(BG_THREADS) resid_gate_bwd_kernel(const void* __restrict__ dout_, int64_t lddout,
+                                                                    const __nv_bfloat16* __restrict__ y, int64_t ldy,
+                                                                    const float* __restrict__ gate,
+                                                                    __nv_bfloat16* __restrict__ dy, int64_t lddy,
+                                                                    float* __restrict__ part, int M, int N, int nparts) {
+  const int col = (blockIdx.y * BG_THREADS + threadIdx.x) * 8;
+  if (col >= N) return;
+  float g[8], ag[8], ab[8];
+  load8_f32(gate + col, g);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) ag[i] = ab[i] = 0.f;
+  for (int64_t row = blockIdx.x; row < M; row += nparts) {
+    float d[8], yv[8], o[8];
+    if constexpr (DOUT_F32) {
+      const float4* p = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(dout_) + row * lddout + col);
+      const float4 a = p[0], b = p[1];
+      d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
+    } else {
+      unpack8(*reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(dout_) + row * lddout + col), d);
+    }
+    unpack8(*reinterpret_cast<const uint4*>(y + row * ldy + col), yv);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[i] = bf16_round(__fmul_rn(d[i], g[i]));
+      ag[i] = __fmaf_rn(d[i], yv[i], ag[i]);
+      ab[i] = __fadd_rn(ab[i], o[i]);
+    }
+    *reinterpret_cast<uint4*>(dy + row * lddy + col) = pack8(o);
+  }
+  float4* dg = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * N + col);
+  float4* db = reinterpret_cast<float4*>(part + (int64_t(nparts) + blockIdx.x) * N + col);
+  dg[0] = make_float4(ag[0], ag[1], ag[2], ag[3]);
+  dg[1] = make_float4(ag[4], ag[5], ag[6], ag[7]);
+  db[0] = make_float4(ab[0], ab[1], ab[2], ab[3]);
+  db[1] = make_float4(ab[4], ab[5], ab[6], ab[7]);
+}
+
+// ------------------------------------------------------------------------------------------
+// LayerNorm + modulation backward (fvb_layernorm_modulate_bwd; arithmetic in include/fvb200.h). The structure of
+// rmsnorm_bwd_kernel: block per row over fixed row sets, the row in registers, mean / variance recomputed from x as the
+// forward does; each thread keeps the fp32 partials sum dn * t and sum dn of its own columns, written to
+// part[0][cta][D] and part[1][cta][D] and added in CTA order by colsum_f32_kernel.
+// ------------------------------------------------------------------------------------------
+template <bool IN_F32, bool GIN_F32>
+__global__ void __launch_bounds__(EW_THREADS) layernorm_modulate_bwd_kernel(
+    const void* __restrict__ x_, int64_t ldx, const __nv_bfloat16* __restrict__ dn, int64_t lddn,
+    const float* __restrict__ gain, int gain_is_scale, int round_ln, const void* __restrict__ gin_, int64_t ldgin,
+    void* __restrict__ dx_, int64_t lddx, float* __restrict__ part, int M, int D, float eps) {
+  __shared__ float red[32];
+  __shared__ float2 red2[32];
+  const int nchunks = D >> 3;
+  float as[EW_MAX_CHUNKS][8], ah[EW_MAX_CHUNKS][8];
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) as[c][i] = ah[c][i] = 0.f;
+  for (int64_t row = blockIdx.x; row < M; row += gridDim.x) {
+    float xv[EW_MAX_CHUNKS][8], dv[EW_MAX_CHUNKS][8];
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        if constexpr (IN_F32) {
+          load8_f32(reinterpret_cast<const float*>(x_) + row * ldx + (ch << 3), xv[c]);
+        } else {
+          unpack8(*reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(x_) + row * ldx + (ch << 3)), xv[c]);
+        }
+        unpack8(*reinterpret_cast<const uint4*>(dn + row * lddn + (ch << 3)), dv[c]);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s += xv[c][i];
+      }
+    }
+    const float mean = block_sum(s, red) / float(D);
+    float q = 0.f;
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float d = xv[c][i] - mean;
+          q += d * d;
+        }
+    }
+    const float rstd = rsqrtf(block_sum(q, red) / float(D) + eps);
+    float2 st = make_float2(0.f, 0.f);  // (sum dt, sum dt * xhat)
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        float gv[8];
+        load8_f32(gain + (ch << 3), gv);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float xh = (xv[c][i] - mean) * rstd;  // the forward's t
+          xv[c][i] = xh;
+          const float dt = __fmul_rn(dv[c][i], gain_is_scale ? __fadd_rn(1.0f, gv[i]) : gv[i]);
+          st.x += dt;
+          st.y = __fmaf_rn(dt, xh, st.y);
+          as[c][i] = __fmaf_rn(dv[c][i], round_ln ? bf16_round(xh) : xh, as[c][i]);
+          ah[c][i] = __fadd_rn(ah[c][i], dv[c][i]);
+        }
+      }
+    }
+    st = block_sum2(st, red2);
+    const float mdt = __fdiv_rn(st.x, float(D)), mdx = __fdiv_rn(st.y, float(D));
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        float gv[8], o[8], gi[8];
+        load8_f32(gain + (ch << 3), gv);
+        if (gin_ != nullptr) {
+          if constexpr (GIN_F32)
+            load8_f32(reinterpret_cast<const float*>(gin_) + row * ldgin + (ch << 3), gi);
+          else
+            unpack8(*reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(gin_) + row * ldgin + (ch << 3)), gi);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float dt = __fmul_rn(dv[c][i], gain_is_scale ? __fadd_rn(1.0f, gv[i]) : gv[i]);
+          o[i] = __fmul_rn(rstd, __fsub_rn(__fsub_rn(dt, mdt), __fmul_rn(xv[c][i], mdx)));
+          if (gin_ != nullptr) o[i] = __fadd_rn(o[i], gi[i]);
+        }
+        if constexpr (IN_F32) {
+          float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(dx_) + row * lddx + (ch << 3));
+          dst[0] = make_float4(o[0], o[1], o[2], o[3]);
+          dst[1] = make_float4(o[4], o[5], o[6], o[7]);
+        } else {
+          *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(dx_) + row * lddx + (ch << 3)) = pack8(o);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+    const int ch = threadIdx.x + c * EW_THREADS;
+    if (ch < nchunks) {
+      float4* ds = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * D + (ch << 3));
+      float4* dh = reinterpret_cast<float4*>(part + (int64_t(gridDim.x) + blockIdx.x) * D + (ch << 3));
+      ds[0] = make_float4(as[c][0], as[c][1], as[c][2], as[c][3]);
+      ds[1] = make_float4(as[c][4], as[c][5], as[c][6], as[c][7]);
+      dh[0] = make_float4(ah[c][0], ah[c][1], ah[c][2], ah[c][3]);
+      dh[1] = make_float4(ah[c][4], ah[c][5], ah[c][6], ah[c][7]);
+    }
+  }
 }
 
 }  // namespace fvb
@@ -971,6 +1183,112 @@ extern "C" int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float*
       reinterpret_cast<const __nv_bfloat16*>(dy), lddy, workspace, M, N, parts);
   FVB_CHECK_CUDA(cudaGetLastError());
   rmsnorm_bwd_dw_kernel<<<(N + 255) / 256, 256, 0, st>>>(workspace, parts, N, reinterpret_cast<__nv_bfloat16*>(db));
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_rmsnorm_rope_bwd_workspace_bytes(int M, int D) { return 2 * fvb_rmsnorm_bwd_workspace_bytes(M, D); }
+
+extern "C" int fvb_rmsnorm_rope_bwd(const void* x0, int64_t ldx0, const void* w0, const void* dy0, int64_t lddy0, void* dx0,
+                                    int64_t lddx0, void* dw0, const void* x1, int64_t ldx1, const void* w1, const void* dy1,
+                                    int64_t lddy1, void* dx1, int64_t lddx1, void* dw1, const float* cos_t, const float* sin_t,
+                                    const int32_t* rope_row, float* workspace, int64_t workspace_bytes, int M, int D,
+                                    int head_dim, float eps, void* stream) {
+  FVB_CHECK_ARG(x0 && w0 && dy0 && dx0 && cos_t && sin_t, "null pointer");
+  FVB_CHECK_ARG(x1 == nullptr || (w1 && dy1 && dx1), "x1 needs w1, dy1 and dx1");
+  FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
+  FVB_CHECK_ARG(head_dim % 8 == 0 && D % head_dim == 0, "head_dim must divide D and be a multiple of 8");
+  FVB_CHECK_ARG(ldx0 % 8 == 0 && lddy0 % 8 == 0 && lddx0 % 8 == 0, "strides must be multiples of 8");
+  FVB_CHECK_ARG(x1 == nullptr || (ldx1 % 8 == 0 && lddy1 % 8 == 0 && lddx1 % 8 == 0), "strides must be multiples of 8");
+  FVB_CHECK_ARG(x1 == nullptr || (dw0 != nullptr) == (dw1 != nullptr), "dw0 and dw1 come together");
+  const int ctas = std::min(M, RB_CTAS);
+  const bool want_dw = dw0 != nullptr;
+  if (want_dw)
+    FVB_CHECK_ARG(workspace != nullptr && workspace_bytes >= fvb_rmsnorm_rope_bwd_workspace_bytes(M, D), "workspace too small");
+  RmsRopeBwdArgs a;
+  a.x[0] = reinterpret_cast<const __nv_bfloat16*>(x0);
+  a.w[0] = reinterpret_cast<const __nv_bfloat16*>(w0);
+  a.dy[0] = reinterpret_cast<const __nv_bfloat16*>(dy0);
+  a.dx[0] = reinterpret_cast<__nv_bfloat16*>(dx0);
+  a.ldx[0] = ldx0;
+  a.lddy[0] = lddy0;
+  a.lddx[0] = lddx0;
+  a.x[1] = reinterpret_cast<const __nv_bfloat16*>(x1);
+  a.w[1] = reinterpret_cast<const __nv_bfloat16*>(w1);
+  a.dy[1] = reinterpret_cast<const __nv_bfloat16*>(dy1);
+  a.dx[1] = reinterpret_cast<__nv_bfloat16*>(dx1);
+  a.ldx[1] = ldx1;
+  a.lddy[1] = lddy1;
+  a.lddx[1] = lddx1;
+  const int nt = x1 != nullptr ? 2 : 1;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  rmsnorm_rope_bwd_kernel<<<dim3(ctas, nt), EW_THREADS, 0, st>>>(a, want_dw ? workspace : nullptr, cos_t, sin_t, rope_row, M, D,
+                                                                 head_dim, eps);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  if (want_dw) {
+    void* dws[2] = {dw0, dw1};
+    for (int t = 0; t < nt; ++t) {
+      rmsnorm_bwd_dw_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace + int64_t(t) * ctas * D, ctas, D,
+                                                             reinterpret_cast<__nv_bfloat16*>(dws[t]));
+      FVB_CHECK_CUDA(cudaGetLastError());
+    }
+  }
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_resid_gate_bwd_workspace_bytes(int M, int N) { return 2 * fvb_bias_grad_bf16_workspace_bytes(M, N); }
+
+extern "C" int fvb_resid_gate_bwd(const void* dout, int dout_is_f32, int64_t lddout, const void* y, int64_t ldy, const float* gate,
+                                  void* dy, int64_t lddy, float* d_gate, void* db, float* workspace, int64_t workspace_bytes,
+                                  int M, int N, void* stream) {
+  FVB_CHECK_ARG(dout && y && gate && dy && d_gate && workspace, "null pointer");
+  FVB_CHECK_ARG(M > 0 && N > 0 && N % 8 == 0, "N must be a positive multiple of 8");
+  FVB_CHECK_ARG(lddout % (dout_is_f32 ? 4 : 8) == 0 && ldy % 8 == 0 && lddy % 8 == 0, "strides must keep rows 16-byte aligned");
+  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gate) & 15) == 0, "gate must be 16-byte aligned");
+  FVB_CHECK_ARG(workspace_bytes >= fvb_resid_gate_bwd_workspace_bytes(M, N), "workspace too small");
+  const int parts = std::min(M, BG_PARTS);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(parts, (N / 8 + BG_THREADS - 1) / BG_THREADS);
+  auto* yb = reinterpret_cast<const __nv_bfloat16*>(y);
+  auto* dyb = reinterpret_cast<__nv_bfloat16*>(dy);
+  if (dout_is_f32)
+    resid_gate_bwd_kernel<true><<<grid, BG_THREADS, 0, st>>>(dout, lddout, yb, ldy, gate, dyb, lddy, workspace, M, N, parts);
+  else
+    resid_gate_bwd_kernel<false><<<grid, BG_THREADS, 0, st>>>(dout, lddout, yb, ldy, gate, dyb, lddy, workspace, M, N, parts);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  colsum_f32_kernel<<<(N + 255) / 256, 256, 0, st>>>(workspace, parts, N, d_gate);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  if (db != nullptr) {
+    rmsnorm_bwd_dw_kernel<<<(N + 255) / 256, 256, 0, st>>>(workspace + int64_t(parts) * N, parts, N, reinterpret_cast<__nv_bfloat16*>(db));
+    FVB_CHECK_CUDA(cudaGetLastError());
+  }
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_layernorm_modulate_bwd_workspace_bytes(int M, int D) { return 2 * fvb_rmsnorm_bwd_workspace_bytes(M, D); }
+
+extern "C" int fvb_layernorm_modulate_bwd(const void* x, int x_is_f32, int64_t ldx, const void* dn, int64_t lddn, const float* gain,
+                                          int gain_is_scale, int round_ln, const void* gin, int gin_is_f32, int64_t ldgin, void* dx,
+                                          int64_t lddx, float* d_gain, float* d_offset, float* workspace, int64_t workspace_bytes,
+                                          int M, int D, float eps, void* stream) {
+  FVB_CHECK_ARG(x && dn && gain && dx && d_gain && d_offset && workspace, "null pointer");
+  FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
+  FVB_CHECK_ARG(ldx % 8 == 0 && lddn % 8 == 0 && lddx % 8 == 0 && (gin == nullptr || ldgin % 8 == 0), "strides must be multiples of 8");
+  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gain) & 15) == 0, "gain must be 16-byte aligned");
+  FVB_CHECK_ARG(workspace_bytes >= fvb_layernorm_modulate_bwd_workspace_bytes(M, D), "workspace too small");
+  FVB_CHECK_ARG(gain_is_scale || !round_ln, "round_ln belongs to the modulation form (the affine forward rounds after w, b)");
+  const int ctas = std::min(M, RB_CTAS);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  auto* dnb = reinterpret_cast<const __nv_bfloat16*>(dn);
+  auto launch = [&](auto kern) {
+    kern<<<ctas, EW_THREADS, 0, st>>>(x, ldx, dnb, lddn, gain, gain_is_scale, round_ln, gin, ldgin, dx, lddx, workspace, M, D, eps);
+  };
+  if (x_is_f32) gin_is_f32 ? launch(layernorm_modulate_bwd_kernel<true, true>) : launch(layernorm_modulate_bwd_kernel<true, false>);
+  else gin_is_f32 ? launch(layernorm_modulate_bwd_kernel<false, true>) : launch(layernorm_modulate_bwd_kernel<false, false>);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  colsum_f32_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace, ctas, D, d_gain);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  colsum_f32_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace + int64_t(ctas) * D, ctas, D, d_offset);
   FVB_CHECK_CUDA(cudaGetLastError());
   return FVB_OK;
 }

@@ -117,6 +117,15 @@ FVB_DEVICE float gelu_tanh_f(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
+FVB_DEVICE float gelu_tanh_grad_f(float x) {
+  // d/dx of gelu_tanh_f, with the same t: 0.5 (1 + t) + 0.5 x (1 - t^2) sqrt(2/pi) (1 + 3 * 0.044715 x^2)
+  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
+  float u = k0 * (x + k1 * x * x * x);
+  float e = ex2(u * 2.885390081777927f);
+  float t = 1.0f - __fdividef(2.0f, e + 1.0f);
+  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * k0 * (1.0f + 3.0f * k1 * x * x);
+}
+
 // W8: the int8 weight tile (BN rows of 64 bytes) sits in the upper half of the stage's bf16 B region
 template <int BN>
 constexpr int W8_STAGING_OFFSET = BN * GEMM_BK;
@@ -179,290 +188,32 @@ FVB_DEVICE float acc_f32(int32_t v) { return __int2float_rn(v); }
 
 // FP8: e4m3 x e4m3 operands; W8: bf16 x int8 (weight-only); I8: int8 x int8 (W8A8); none: bf16 x bf16.
 // TA / TB: A / B is MN-major (bf16 x bf16 only).
+// Epilogue of the dgrad GEMM only (fvb_linear_dgrad_gelu_bf16): dx = bf16(bf16(acc) * gelu_tanh'(h)), h read through resid.
+constexpr int EPI_DGELU_TANH = 100;
+
+// fvb_linear_bf16_aux: the bf16 y = bf16(acc + bias) of every element is also stored to aux[row * ldaux + col]. A template
+// so that the kernel body's e4m3 / int8 branches, discarded for it, stay dependent.
+template <bool SCALED = false>
+struct GemmParamsAuxT : GemmParams {
+  __nv_bfloat16* aux;
+  int64_t ldaux;
+};
+using GemmParamsAux = GemmParamsAuxT<>;
+
 template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false, bool TA = false, bool TB = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParamsT<FP8 || W8 || I8> p) {
-  static_assert(!((TA || TB) && (FP8 || W8 || I8)), "transposed operands are bf16 only: e4m3 / s8 wgmma has no transpose bits");
-  static_assert(TB || !TA, "the transposed producer loads B MN-major: TA comes with TB (wgrad)");
-  using Cfg = GemmCfg<BN>;
-  constexpr int BK = FP8 || I8 ? GEMM_BK_FP8 : GEMM_BK;
-  using Acc = std::conditional_t<I8, int32_t, float>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::STAGES;
+  constexpr bool AUX = false;
+#include "gemm_kernel_body.cuh"
+}
 
-  const int wg = threadIdx.x >> 7;
-  const int tiles_per_batch = p.num_m * p.num_n;
-  const int num_tiles = tiles_per_batch * p.batch;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 8);  // lane 0 of each of the eight consumer warps
-    }
-    if constexpr (W8)
-      for (int i = 0; i < Cfg::STAGES; ++i) mbar_init(&bars[2 * Cfg::STAGES + i], 1);  // `landed` below
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    reg_dealloc<40>();
-    if constexpr (W8) {
-      // thread 0 issues the TMA loads onto `landed`; warps 1-3 widen each landed weight tile, then release the stage to
-      // the consumers on `full`
-      uint64_t* landed = bars + 2 * Cfg::STAGES;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        const int bt = tile / tiles_per_batch;
-        tile_coords(tile - bt * tiles_per_batch, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
-        for (int kb = 0; kb < p.num_k; ++kb) {
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          if (threadIdx.x == 0) {
-            mbar_wait(&empty[stage], phase ^ 1);
-            mbar_expect_tx(&landed[stage], Cfg::A_BYTES + BN * GEMM_BK);
-            const int k0 = kb * GEMM_BK;
-            const int seg = k0 / p.a_seg_len;
-            tma_load_4d(sa, &tmA, &landed[stage], k0 - seg * p.a_seg_len, m_blk * GEMM_BM, seg, bt);
-            tma_load_3d(sb + W8_STAGING_OFFSET<BN>, &tmB, &landed[stage], k0, n_blk * BN, bt);
-          } else if (threadIdx.x >= 32) {
-            mbar_wait(&landed[stage], phase);
-            w8_widen_tile<BN>(smem_u32(sb), threadIdx.x - 32);
-            fence_proxy_async();  // the generic-proxy stores are read by wgmma (async proxy)
-            named_bar_sync(1, W8_CONVERT_THREADS);
-            if (threadIdx.x == 32) mbar_arrive(&full[stage]);
-          }
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-      return;
-    }
-    if constexpr (TA || TB) {
-      // MN-major operands: one 2-D TMA per 64-wide chunk ([K][MN] maps; MN and K tails zero-filled), chunk-major in the stage.
-      // A K-major A (TB only) is the forward's 4-D load.
-      if (threadIdx.x == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-          int m_blk, n_blk;
-          tile_coords(tile, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
-          for (int kb = 0; kb < p.num_k; ++kb) {
-            mbar_wait(&empty[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-            uint8_t* sb = sa + Cfg::A_BYTES;
-            mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-            if constexpr (TA) {
-#pragma unroll
-              for (int c = 0; c < GEMM_BM / GEMM_MN_CHUNK; ++c)
-                tma_load_2d(sa + c * GEMM_MN_CHUNK_BYTES, &tmA, &full[stage], m_blk * GEMM_BM + c * GEMM_MN_CHUNK, kb * BK);
-            } else {
-              tma_load_4d(sa, &tmA, &full[stage], kb * BK, m_blk * GEMM_BM, 0, 0);
-            }
-#pragma unroll
-            for (int c = 0; c < BN / GEMM_MN_CHUNK; ++c)
-              tma_load_2d(sb + c * GEMM_MN_CHUNK_BYTES, &tmB, &full[stage], n_blk * BN + c * GEMM_MN_CHUNK, kb * BK);
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-        }
-      }
-      return;
-    }
-    if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        const int bt = tile / tiles_per_batch;
-        tile_coords(tile - bt * tiles_per_batch, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
-        for (int kb = 0; kb < p.num_k; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          mbar_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-          {
-            const int k0 = kb * BK;
-            const int seg = k0 / p.a_seg_len;
-            tma_load_4d(sa, &tmA, &full[stage], k0 - seg * p.a_seg_len, m_blk * GEMM_BM, seg, bt);
-          }
-          tma_load_3d(sb, &tmB, &full[stage], kb * BK, n_blk * BN, bt);
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-    return;
-  }
-  // ------------------------------ MMA + epilogue (rows [64 (wg - 1), 64 wg) of the tile) ------------------------------
-  reg_alloc<232>();  // 128 x 40 + 256 x 232 = 64 512 of 65 536 registers
-  const int half = wg - 1;
-  const int warp = (threadIdx.x >> 5) & 3;
-  const int lane = threadIdx.x & 31;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    int m_blk, n_blk;
-    const int bt = tile / tiles_per_batch;
-    tile_coords(tile - bt * tiles_per_batch, p.num_m, p.num_n, p.stripe_n, m_blk, n_blk);
-    Acc acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = Acc(0);
-    int prev = -1;
-    if constexpr (FP8) {
-      // per k-block partial sums in `part` (the first MMA overwrites it), promoted into the fp32 accumulators after the
-      // k-block's MMAs complete; the other consumer warpgroup keeps the tensor cores busy meanwhile
-      float part[BN / 2];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) part[i] = 0.f;
-      for (int kb = 0; kb < p.num_k; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + half * (64 * 128);
-        const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
-        const uint64_t da = make_desc_kmajor_sw128(sa);
-        const uint64_t db = make_desc_kmajor_sw128(sb);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK_FP8 / 32; ++k) wgmma_ss_e4m3<BN>(part, da + uint64_t(2 * k), db + uint64_t(2 * k), k);
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(part);
-        if (lane == 0) mbar_arrive(&empty[stage]);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = __fadd_rn(acc[i], part[i]);
-        if (++stage == Cfg::STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    } else {
-    for (int kb = 0; kb < p.num_k; ++kb) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + half * (64 * 128);
-      const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
-      const uint64_t da = make_desc_kmajor_sw128(sa);
-      const uint64_t db = make_desc_kmajor_sw128(sb);
-      wgmma_fence();
-      if constexpr (I8) {
-#pragma unroll
-        for (int k = 0; k < GEMM_BK_FP8 / 32; ++k) wgmma_ss_s8<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), 1);
-      } else if constexpr (TA || TB) {
-        // MN-major: this warpgroup's 64 A rows are chunk `half` (the same +8 KB as the K-major half); chunks are 8 KB apart
-        // (LBO), 8-row k groups 1024 B (SBO); a k16 step is 16 rows of 128 B (+128 on the descriptor)
-        const uint64_t ta = TA ? make_desc_mnmajor_sw128(sa, GEMM_MN_CHUNK_BYTES) : da;
-        const uint64_t tb = TB ? make_desc_mnmajor_sw128(sb, GEMM_MN_CHUNK_BYTES) : db;
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k)
-          wgmma_ss_trans<BN, TA, TB>(acc, ta + uint64_t(k * (TA ? 128 : 2)), tb + uint64_t(k * (TB ? 128 : 2)));
-      } else {
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, da + uint64_t(2 * k), db + uint64_t(2 * k));
-      }
-      wgmma_commit();
-      // keep one k-block of MMAs in flight: the stage read by the previous group is free once it completes
-      wgmma_wait<1>();
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-      prev = stage;
-      if (++stage == Cfg::STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-    }
-
-    // ------------------------------ epilogue ------------------------------
-    const int row0 = m_blk * GEMM_BM + half * 64 + warp * 16 + (lane >> 2);
-    const float* gate_rows_p[2] = {p.gate, p.gate};
-    if constexpr (EPI != FVB_EPI_RESID_BF16)
-      if (p.gate_rows > 0)
-        for (int i = 0; i < 2; ++i) gate_rows_p[i] += int64_t((row0 + 8 * i) / p.gate_rows) * p.gate_stride;
-    float sx[2] = {1.f, 1.f};
-    if constexpr (FP8 || I8)
-      for (int i = 0; i < 2; ++i) sx[i] = row0 + 8 * i < p.M ? __ldg(p.a_scale + row0 + 8 * i) : 0.f;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = n_blk * BN + 8 * j + 2 * (lane & 3);
-      if (col >= p.N) continue;  // N is a multiple of 8: the pair (col, col + 1) is inside or outside together
-      const int64_t out_col = p.out_col_offsets ? __ldg(p.out_col_offsets + (col >> 7)) + (col & 127) : int64_t(col);
-      float2 bf = make_float2(0.f, 0.f);
-      if (p.bias != nullptr) bf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
-      float2 sw = make_float2(1.f, 1.f);
-      if constexpr (FP8 || W8 || I8) {
-        sw.x = col < p.N_valid ? __ldg(p.b_scale + col) : 0.f;
-        sw.y = col + 1 < p.N_valid ? __ldg(p.b_scale + col + 1) : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = row0 + 8 * i;
-        if (row >= p.M) continue;
-        // I8: float(acc) rounds to nearest (exact up to 2^24)
-        float f0 = acc_f32(acc[4 * j + 2 * i]), f1 = acc_f32(acc[4 * j + 2 * i + 1]);
-        if constexpr (FP8 || I8) {  // (acc * s_x[m]) * s_w[n], fp32 round-to-nearest, before the bias
-          f0 = __fmul_rn(__fmul_rn(f0, sx[i]), sw.x);
-          f1 = __fmul_rn(__fmul_rn(f1, sx[i]), sw.y);
-        } else if constexpr (W8) {  // acc * s_w[n], fp32 round-to-nearest, before the bias
-          f0 = __fmul_rn(f0, sw.x);
-          f1 = __fmul_rn(f1, sw.y);
-        }
-        if (p.bias != nullptr) {
-          f0 = __fadd_rn(f0, bf.x);
-          f1 = __fadd_rn(f1, bf.y);
-        }
-        // y = bf16(acc + bias) in every mode (the reference's F.linear output dtype)
-        if constexpr (EPI == FVB_EPI_BIAS_GELU_TANH) {
-          f0 = gelu_tanh_f(bf16_round(f0));
-          f1 = gelu_tanh_f(bf16_round(f1));
-        } else if constexpr (EPI == FVB_EPI_DIV) {
-          f0 = __fdiv_rn(bf16_round(f0), p.div);
-          f1 = __fdiv_rn(bf16_round(f1), p.div);
-        } else if constexpr (EPI == FVB_EPI_SCALE_F32) {
-          f0 = __fmul_rn(f0, p.div);
-          f1 = __fmul_rn(f1, p.div);
-        } else if constexpr (EPI == FVB_EPI_RESID_GATE_F32 || EPI == FVB_EPI_RESID_GATE_BF16 ||
-                             EPI == FVB_EPI_RESID_GATE_BF16R || EPI == FVB_EPI_RESID_BF16) {
-          const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.resid + int64_t(row) * p.ldr + col));
-          const float y0 = bf16_round(f0), y1 = bf16_round(f1);
-          if constexpr (EPI == FVB_EPI_RESID_BF16) {
-            f0 = __fadd_rn(rf.x, y0);
-            f1 = __fadd_rn(rf.y, y1);
-          } else {
-            const float2 g = *reinterpret_cast<const float2*>(gate_rows_p[i] + col);
-            if constexpr (EPI == FVB_EPI_RESID_GATE_BF16R) {
-              f0 = __fadd_rn(rf.x, bf16_round(__fmul_rn(y0, g.x)));
-              f1 = __fadd_rn(rf.y, bf16_round(__fmul_rn(y1, g.y)));
-            } else {
-              f0 = __fadd_rn(rf.x, __fmul_rn(y0, g.x));
-              f1 = __fadd_rn(rf.y, __fmul_rn(y1, g.y));
-            }
-          }
-        }
-        if constexpr (EPI == FVB_EPI_RESID_GATE_F32 || EPI == FVB_EPI_SCALE_F32) {
-          float* op = reinterpret_cast<float*>(p.out) + int64_t(bt) * p.out_batch_stride + int64_t(row) * p.ldo + out_col;
-          *reinterpret_cast<float2*>(op) = make_float2(f0, f1);
-        } else {
-          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + int64_t(bt) * p.out_batch_stride + int64_t(row) * p.ldo + out_col;
-          *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(f0, f1);
-        }
-      }
-    }
-  }
+template <int BN, int EPI, bool FP8 = false, bool W8 = false, bool I8 = false, bool TA = false, bool TB = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_aux_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const GemmParamsAuxT<FP8 || W8 || I8> p) {
+  static_assert(!(FP8 || W8 || I8 || TA || TB), "the aux epilogues are bf16 forward GEMMs");
+  constexpr bool AUX = true;
+#include "gemm_kernel_body.cuh"
 }
 
 template <int BN, int EPI, bool FP8, bool W8 = false, bool I8 = false, bool TA = false, bool TB = false>
@@ -496,6 +247,33 @@ static int dispatch_epi(int epi, const CUtensorMap& a, const CUtensorMap& b, con
   return set_error(FVB_ERR_INVALID_ARG, "unknown epilogue%s");
 }
 
+template <int BN, int EPI>
+static int launch_gemm_aux(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParamsAux& p, cudaStream_t st) {
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_aux_kernel<BN, EPI>;
+  static bool configured = false;
+  if (!configured) {
+    FVB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    configured = true;
+  }
+  const int tiles = p.num_m * p.num_n;
+  const int grid = tiles < sm_count() ? tiles : sm_count();
+  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, p);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+// bf16 operands with the pre-epilogue y also stored (fvb_linear_bf16_aux): the epilogues whose y the block backward needs
+template <int BN>
+static int dispatch_epi_aux(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsAux& p, cudaStream_t st) {
+  switch (epi) {
+    case FVB_EPI_BIAS_GELU_TANH: return launch_gemm_aux<BN, FVB_EPI_BIAS_GELU_TANH>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_F32: return launch_gemm_aux<BN, FVB_EPI_RESID_GATE_F32>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16: return launch_gemm_aux<BN, FVB_EPI_RESID_GATE_BF16>(a, b, p, st);
+  }
+  return set_error(FVB_ERR_INVALID_ARG, "fvb_linear_bf16_aux takes FVB_EPI_BIAS_GELU_TANH, _RESID_GATE_F32 or _RESID_GATE_BF16%s");
+}
+
 // fp8 / int8 operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)
 template <int BN, bool FP8, bool W8, bool I8 = false>
 static int dispatch_epi_scaled(int epi, const CUtensorMap& a, const CUtensorMap& b, const GemmParamsFp8& p, cudaStream_t st) {
@@ -519,7 +297,7 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
                      const void* resid, int64_t ldr,
                      const float* gate, int gate_rows, int64_t gate_stride, float div, int M, int N, int K, int batch,
                      int epilogue, void* stream, const float* x_scale = nullptr, const float* w_scale = nullptr,
-                     bool int8_operands = false) {
+                     bool int8_operands = false, void* aux = nullptr, int64_t ldaux = 0) {
   // x_scale / w_scale set: x and w are e4m3 (one byte per element) with per-row / per-output-channel fp32 scales, or
   // int8 with the same scales when int8_operands is set.
   // w_scale alone: x is bf16 and w is int8 with per-output-channel fp32 scales.
@@ -625,6 +403,15 @@ static int gemm_impl(const void* x, int64_t ldx, int64_t x_batch, int a_seg_len,
     p.stripe_n = 0;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (aux != nullptr) {
+    GemmParamsAux pa;
+    static_cast<GemmParams&>(pa) = p;
+    pa.aux = reinterpret_cast<__nv_bfloat16*>(aux);
+    pa.ldaux = ldaux;
+    if (BN == 256) return dispatch_epi_aux<256>(epilogue, tmA, tmB, pa, st);
+    if (BN == 128) return dispatch_epi_aux<128>(epilogue, tmA, tmB, pa, st);
+    return dispatch_epi_aux<64>(epilogue, tmA, tmB, pa, st);
+  }
   if (fp8)
     return BN == 128 ? dispatch_epi_scaled<128, true, false>(epilogue, tmA, tmB, p, st)
                      : dispatch_epi_scaled<64, true, false>(epilogue, tmA, tmB, p, st);
@@ -649,6 +436,15 @@ extern "C" int fvb_linear_bf16(const void* x, int64_t ldx, const void* w, int64_
   if (epilogue == FVB_EPI_DIV) return set_error(FVB_ERR_INVALID_ARG, "use fvb_gemm_batched_bf16 for FVB_EPI_DIV%s");
   return gemm_impl(x, ldx, 0, 0, 0, w, ldw, 0, bias, out, ldo, 0, nullptr, resid, ldr, gate, gate_rows, gate_stride, 1.0f,
                    M, N, K, 1, epilogue, stream);
+}
+
+extern "C" int fvb_linear_bf16_aux(const void* x, int64_t ldx, const void* w, int64_t ldw, const void* bias, void* out,
+                                   int64_t ldo, const void* resid, int64_t ldr, const float* gate, int gate_rows,
+                                   int64_t gate_stride, void* aux, int64_t ldaux, int M, int N, int K, int epilogue, void* stream) {
+  FVB_CHECK_ARG(aux != nullptr && ldaux % 8 == 0 && ldaux >= N, "aux required (ldaux a multiple of 8, >= N)");
+  FVB_CHECK_ARG(N % 8 == 0, "N must be a multiple of 8");
+  return gemm_impl(x, ldx, 0, 0, 0, w, ldw, 0, bias, out, ldo, 0, nullptr, resid, ldr, gate, gate_rows, gate_stride, 1.0f,
+                   M, N, K, 1, epilogue, stream, nullptr, nullptr, false, aux, ldaux);
 }
 
 extern "C" int fvb_linear_bf16_sp(const void* x, int64_t ldx, int x_seg_len, int64_t x_seg_stride, const void* w,
@@ -712,13 +508,18 @@ extern "C" int fvb_linear_w8a8_sp(const void* xq, int64_t ldx, const float* x_sc
 // ------------------------------------------------------------------------------------------------------------------------
 template <bool TA>
 static int dispatch_bwd(int BN, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, cudaStream_t st) {
+  if (p.resid != nullptr) {  // dgrad with the GELU-backward epilogue
+    if (BN == 256) return launch_gemm<256, EPI_DGELU_TANH, false, false, false, false, true>(a, b, p, st);
+    if (BN == 128) return launch_gemm<128, EPI_DGELU_TANH, false, false, false, false, true>(a, b, p, st);
+    return launch_gemm<64, EPI_DGELU_TANH, false, false, false, false, true>(a, b, p, st);
+  }
   if (BN == 256) return launch_gemm<256, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
   if (BN == 128) return launch_gemm<128, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
   return launch_gemm<64, FVB_EPI_BIAS, false, false, false, TA, true>(a, b, p, st);
 }
 
 static int gemm_bwd_impl(bool a_mn_major, const void* a, int64_t lda, const void* b, int64_t ldb, void* out, int64_t ldo,
-                         int Mo, int No, int R, bool weight_stripes, void* stream) {
+                         int Mo, int No, int R, bool weight_stripes, void* stream, const void* h = nullptr, int64_t ldh = 0) {
   FVB_CHECK_ARG(a && b && out, "null pointer");
   FVB_CHECK_ARG(Mo > 0 && No > 0 && R > 0, "empty problem");
   FVB_CHECK_ARG(No % 8 == 0, "output columns (K of the forward) must be a multiple of 8");
@@ -749,6 +550,8 @@ static int gemm_bwd_impl(bool a_mn_major, const void* a, int64_t lda, const void
   GemmParams p{};
   p.out = out;
   p.ldo = ldo;
+  p.resid = reinterpret_cast<const __nv_bfloat16*>(h);
+  p.ldr = ldh;
   p.a_seg_len = R;
   p.div = 1.f;
   p.M = Mo;
@@ -763,7 +566,8 @@ static int gemm_bwd_impl(bool a_mn_major, const void* a, int64_t lda, const void
   // each k-block of dy and x is read from HBM once per wave and shared through L2 by 16 resp. 8 CTAs.
   p.stripe_n = weight_stripes && p.num_m >= 16 && p.num_n > 8 ? 8 : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return a_mn_major ? dispatch_bwd<true>(BN, tmA, tmB, p, st) : dispatch_bwd<false>(BN, tmA, tmB, p, st);
+  if (a_mn_major) return dispatch_bwd<true>(BN, tmA, tmB, p, st);
+  return dispatch_bwd<false>(BN, tmA, tmB, p, st);
 }
 
 extern "C" int fvb_linear_dgrad_bf16(const void* dy, int64_t lddy, const void* w, int64_t ldw, void* dx, int64_t lddx, int M,
@@ -776,4 +580,11 @@ extern "C" int fvb_linear_wgrad_bf16(const void* dy, int64_t lddy, const void* x
                                      int N, int K, void* stream) {
   // dw[N, K] = dy^T . x over the M tokens: A = dy^T (MN-major: token row m holds the N output rows), B = x (MN-major)
   return gemm_bwd_impl(true, dy, lddy, x, ldx, dw, lddw, N, K, M, false, stream);
+}
+
+extern "C" int fvb_linear_dgrad_gelu_bf16(const void* dy, int64_t lddy, const void* w, int64_t ldw, const void* h, int64_t ldh,
+                                          void* dh, int64_t lddh, int M, int N, int K, void* stream) {
+  // fvb_linear_dgrad_bf16 with h[M, K] (the fc_in output before its GELU) read in the epilogue
+  FVB_CHECK_ARG(h != nullptr && ldh % 8 == 0, "h required (ldh a multiple of 8)");
+  return gemm_bwd_impl(false, dy, lddy, w, ldw, dh, lddh, M, K, N, true, stream, h, ldh);
 }

@@ -244,7 +244,8 @@ class SPWanDiT:
 
     def block_forward(self, x, blk, ctx, temb6, lay, plan_t, rope_row_local):
         from . import ops, vsa
-        from .wan_dit import Modulation, block_tail
+        from .wan_dit import Modulation, block_tail, refuse_grad
+        refuse_grad("SPWanDiT", blk, x, ctx, temb6)
         plan, qkv_off, head_off = plan_t
         cfg = self.m.cfg
         D, d, Hl, P = cfg.hidden_size, cfg.head_dim, plan.local_heads, self.world

@@ -91,6 +91,131 @@ def linear_bwd(x: torch.Tensor, w: torch.Tensor, dy: torch.Tensor, need_dx: bool
     return dx, dw, db
 
 
+def _check_2d(t: torch.Tensor, name: str, shape, dtypes=(torch.bfloat16,)) -> None:
+    if not t.is_cuda or t.dtype not in dtypes or t.dim() != 2 or t.stride(1) != 1 or tuple(t.shape) != tuple(shape):
+        raise FvbError(f"{name} must be a CUDA {'/'.join(map(str, dtypes))} [{shape[0]}, {shape[1]}] view with unit inner stride")
+
+
+def linear_aux(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, epilogue: int,
+               resid: torch.Tensor | None = None, gate: torch.Tensor | None = None, gate_rows: int = 0):
+    """fvb_linear_bf16_aux: `linear` (bf16 weight, EPI_BIAS_GELU_TANH / EPI_RESID_GATE_F32 / EPI_RESID_GATE_BF16) that also
+    returns the bf16 y = bf16(x @ w.T + bias) its epilogue consumes. x: [M, K] with unit inner stride; one gate vector
+    (gate_rows 0). Returns (out, aux); out has the bits of `linear`, aux those of `linear` with EPI_BIAS."""
+    if gate_rows != 0:
+        raise FvbError("linear_aux takes one gate vector for all rows (gate_rows=0)")
+    _require_cuda_bf16(x, "x")
+    _require_cuda_bf16(w, "w")
+    if x.dim() != 2 or x.stride(1) != 1 or w.stride(1) != 1:
+        raise FvbError("linear_aux: x [M, K] and w [N, K] with unit inner stride")
+    M, K = x.shape
+    N = w.shape[0]
+    out = torch.empty((M, N), dtype=torch.float32 if epilogue == EPI_RESID_GATE_F32 else torch.bfloat16, device=x.device)
+    aux = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
+    if resid is not None:
+        _check_2d(resid, "resid", (M, N))
+    gate_stride = _check_grouped(gate, N, 0, M, "gate")
+    if bias is not None:
+        _require_cuda_bf16(bias, "bias")
+        assert bias.is_contiguous() and bias.numel() == N
+    check(lib().fvb_linear_bf16_aux(ptr(x), c_int64(x.stride(0)), ptr(w), c_int64(w.stride(0)), ptr(bias), ptr(out),
+                                    c_int64(N), ptr(resid), c_int64(resid.stride(0) if resid is not None else 0), _f32p(gate),
+                                    c_int(0), c_int64(gate_stride), ptr(aux), c_int64(N), c_int(M), c_int(N), c_int(K),
+                                    c_int(epilogue), stream_ptr()))
+    return out, aux
+
+
+def linear_dgrad_gelu(dy: torch.Tensor, w: torch.Tensor, h: torch.Tensor) -> torch.Tensor:
+    """fvb_linear_dgrad_gelu_bf16: dh = bf16(bf16(dy @ w) * gelu_tanh'(h)) for y = gelu_tanh(h) @ w.T (+ b). dy [M, N],
+    w [N, K], h [M, K] bf16 2-D views with unit inner stride. Returns dh [M, K]."""
+    M, N = dy.shape
+    K = w.shape[1]
+    _check_2d(dy, "dy", (M, N))
+    _check_2d(w, "w", (N, K))
+    _check_2d(h, "h", (M, K))
+    dh = torch.empty((M, K), dtype=torch.bfloat16, device=dy.device)
+    check(lib().fvb_linear_dgrad_gelu_bf16(ptr(dy), c_int64(dy.stride(0)), ptr(w), c_int64(w.stride(0)), ptr(h),
+                                           c_int64(h.stride(0)), ptr(dh), c_int64(K), c_int(M), c_int(N), c_int(K), stream_ptr()))
+    return dh
+
+
+def resid_gate_bwd(dout: torch.Tensor, y: torch.Tensor, gate: torch.Tensor, need_db: bool = True):
+    """fvb_resid_gate_bwd: backward of out = resid + y * gate (EPI_RESID_GATE_F32 / _BF16). dout fp32 or bf16 [M, N], y the
+    saved bf16 [M, N] (2-D views, unit inner stride), gate fp32 [N]. Returns (dy bf16 [M, N], d_gate fp32 [N], db bf16 [N] or
+    None); the residual's gradient is dout."""
+    M, N = y.shape
+    _check_2d(dout, "dout", (M, N), (torch.float32, torch.bfloat16))
+    _check_2d(y, "y", (M, N))
+    if gate.dtype != torch.float32 or not gate.is_contiguous() or gate.numel() != N:
+        raise FvbError(f"resid_gate_bwd: gate must be a contiguous fp32 [{N}] tensor")
+    dy = torch.empty((M, N), dtype=torch.bfloat16, device=y.device)
+    d_gate = torch.empty(N, dtype=torch.float32, device=y.device)
+    db = torch.empty(N, dtype=torch.bfloat16, device=y.device) if need_db else None
+    ws = _workspace(int(lib().fvb_resid_gate_bwd_workspace_bytes(c_int(M), c_int(N))), y.device)
+    check(lib().fvb_resid_gate_bwd(ptr(dout), c_int(int(dout.dtype == torch.float32)), c_int64(dout.stride(0)), ptr(y),
+                                   c_int64(y.stride(0)), _f32p(gate), ptr(dy), c_int64(N), _f32p(d_gate), ptr(db), _f32p(ws),
+                                   c_int64(ws.numel()), c_int(M), c_int(N), stream_ptr()))
+    return dy, d_gate, db
+
+
+def layernorm_modulate_bwd(x: torch.Tensor, dn: torch.Tensor, scale: torch.Tensor | None = None,
+                           weight: torch.Tensor | None = None, round_ln: bool = False, gin: torch.Tensor | None = None,
+                           eps: float = 1e-6):
+    """fvb_layernorm_modulate_bwd: backward of layernorm_modulate(x, scale, shift, round_ln=...) (scale given) or of
+    layernorm_modulate(x, weight=weight, bias=...) (weight given), one (scale, shift) for all rows. x bf16 or fp32 [M, D],
+    dn bf16 [M, D]; gin: optional fp32 / bf16 [M, D] gradient added into dx. Returns (dx in x's dtype, d_scale or d_weight
+    fp32 [D], d_shift or d_bias fp32 [D])."""
+    M, D = x.shape
+    _check_2d(x, "x", (M, D), (torch.float32, torch.bfloat16))
+    _check_2d(dn, "dn", (M, D))
+    if (scale is None) == (weight is None):
+        raise FvbError("layernorm_modulate_bwd takes scale (modulation) or weight (affine), not both")
+    if round_ln and weight is not None:
+        raise FvbError("layernorm_modulate_bwd: round_ln is the modulation form's (the affine forward rounds after w, b)")
+    gain = scale if scale is not None else weight
+    if gain.dtype != torch.float32 or not gain.is_contiguous() or gain.numel() != D:
+        raise FvbError(f"layernorm_modulate_bwd: scale / weight must be a contiguous fp32 [{D}] tensor")
+    if gin is not None:
+        _check_2d(gin, "gin", (M, D), (torch.float32, torch.bfloat16))
+    dx = torch.empty((M, D), dtype=x.dtype, device=x.device)
+    d_gain = torch.empty(D, dtype=torch.float32, device=x.device)
+    d_off = torch.empty(D, dtype=torch.float32, device=x.device)
+    ws = _workspace(int(lib().fvb_layernorm_modulate_bwd_workspace_bytes(c_int(M), c_int(D))), x.device)
+    check(lib().fvb_layernorm_modulate_bwd(ptr(x), c_int(int(x.dtype == torch.float32)), c_int64(x.stride(0)), ptr(dn),
+                                           c_int64(dn.stride(0)), _f32p(gain), c_int(int(scale is not None)), c_int(int(round_ln)),
+                                           ptr(gin), c_int(int(gin is not None and gin.dtype == torch.float32)),
+                                           c_int64(gin.stride(0) if gin is not None else 0), ptr(dx), c_int64(D), _f32p(d_gain),
+                                           _f32p(d_off), _f32p(ws), c_int64(ws.numel()), c_int(M), c_int(D), c_float(eps),
+                                           stream_ptr()))
+    return dx, d_gain, d_off
+
+
+def rmsnorm_rope_bwd(x0, w0, dy0, dx0, x1, w1, dy1, dx1, cos, sin, rope_row=None, head_dim: int = 128, eps: float = 1e-6,
+                     want_dw: bool = True):
+    """fvb_rmsnorm_rope_bwd: backward of rmsnorm_rope_(x0, w0, x1, w1, cos, sin, rope_row) (bf16 weights) into dx0 / dx1,
+    which may be column slices of a fused gradient buffer. x*, dy*, dx*: bf16 [M, D] 2-D views with unit inner stride (x1 /
+    dy1 / dx1 None: one tensor); cos / sin fp32 [S_pos, head_dim]. Returns (dw0, dw1) bf16 [D] (None without want_dw)."""
+    M, D = x0.shape
+    for n, t in (("x0", x0), ("dy0", dy0), ("dx0", dx0)) + ((("x1", x1), ("dy1", dy1), ("dx1", dx1)) if x1 is not None else ()):
+        _check_2d(t, n, (M, D))
+    for n, w in (("w0", w0), ("w1", w1 if x1 is not None else w0)):
+        if w.dtype != torch.bfloat16 or not w.is_contiguous() or w.numel() != D:
+            raise FvbError(f"rmsnorm_rope_bwd: {n} must be a contiguous bf16 [{D}] tensor (fp32 RMSNorm weights have no backward)")
+    if cos.dtype != torch.float32 or sin.dtype != torch.float32 or not cos.is_contiguous() or not sin.is_contiguous():
+        raise FvbError("rmsnorm_rope_bwd: cos / sin must be contiguous fp32 tables")
+    if rope_row is not None:
+        _check_i32(rope_row, "rope_row", M)
+    dw0 = torch.empty(D, dtype=torch.bfloat16, device=x0.device) if want_dw else None
+    dw1 = torch.empty(D, dtype=torch.bfloat16, device=x0.device) if want_dw and x1 is not None else None
+    ws = _workspace(int(lib().fvb_rmsnorm_rope_bwd_workspace_bytes(c_int(M), c_int(D))), x0.device) if want_dw else None
+    ld = lambda t: c_int64(t.stride(0) if t is not None else 0)
+    check(lib().fvb_rmsnorm_rope_bwd(ptr(x0), ld(x0), ptr(w0), ptr(dy0), ld(dy0), ptr(dx0), ld(dx0), ptr(dw0), ptr(x1), ld(x1),
+                                     ptr(w1 if x1 is not None else None), ptr(dy1), ld(dy1), ptr(dx1), ld(dx1), ptr(dw1),
+                                     _f32p(cos), _f32p(sin), _i32p(rope_row), _f32p(ws),
+                                     c_int64(ws.numel() if ws is not None else 0), c_int(M), c_int(D), c_int(head_dim),
+                                     c_float(eps), stream_ptr()))
+    return dw0, dw1
+
+
 FP8_E4M3_MAX = 448.0
 
 

@@ -159,6 +159,7 @@ class WanBlock:
         self.w_1, self.b_1 = bf(g("ffn.fc_in.weight")), bf(g("ffn.fc_in.bias"))
         self.w_2, self.b_2 = bf(g("ffn.fc_out.weight")), bf(g("ffn.fc_out.bias"))
         self.scale_shift_table = g("scale_shift_table")  # dtype as loaded: the modulation sum happens in torch
+        self.trainable = not (cfg.fp8_linears or cfg.int8_weights)
         if cfg.fp8_linears:
             for n in FP8_LINEARS:  # replacing the attribute drops the block's bf16 copy
                 setattr(self, n, ops.Fp8Weight.quantize(getattr(self, n)))
@@ -166,6 +167,43 @@ class WanBlock:
             for n in INT8_LINEARS:
                 if getattr(self, n) is not None:
                     setattr(self, n, ops.Int8Weight.quantize(getattr(self, n), cfg.int8_activations))
+
+
+    def tensors(self) -> dict:
+        """The block's trainable tensors in its own fused layout, by attribute name (every one a leaf an optimizer can
+        step; w_kv_img / b_kv_img / norm_k_img only on I2V blocks). `to_reference_names` maps this dict, or one of their
+        .grad, back to the reference parameter names."""
+        names = ["w_qkv", "b_qkv", "norm_q", "norm_k", "w_o", "b_o", "norm2_w", "norm2_b", "w_q2", "b_q2", "w_kv2", "b_kv2",
+                 "norm_q2", "norm_k2", "w_o2", "b_o2", "w_1", "b_1", "w_2", "b_2", "scale_shift_table"]
+        if self.w_kv_img is not None:
+            names += ["w_kv_img", "b_kv_img", "norm_k_img"]
+        return {n: getattr(self, n) for n in names}
+
+    @staticmethod
+    def to_reference_names(t: dict, prefix: str = "") -> dict:
+        """{fused name: tensor} (WanBlock.tensors(), or the same keys holding gradients) -> {reference name: tensor}: the
+        fused QKV(+gate) / text KV / image KV rows are split back into their projections (views, no copies)."""
+        out = {}
+        D = t["w_o"].shape[0]
+        qkv = ["to_q", "to_k", "to_v", "to_gate_compress"][:t["w_qkv"].shape[0] // D]
+        for i, n in enumerate(qkv):
+            out[n + ".weight"] = t["w_qkv"][i * D:(i + 1) * D]
+            out[n + ".bias"] = t["b_qkv"][i * D:(i + 1) * D]
+        for src, dst in (("w_kv2", "attn2.to_{}.weight"), ("b_kv2", "attn2.to_{}.bias")):
+            out[dst.format("k")], out[dst.format("v")] = t[src][:D], t[src][D:]
+        if "w_kv_img" in t:
+            for src, dst in (("w_kv_img", "attn2.add_{}_proj.weight"), ("b_kv_img", "attn2.add_{}_proj.bias")):
+                out[dst.format("k")], out[dst.format("v")] = t[src][:D], t[src][D:]
+            out["attn2.norm_added_k.weight"] = t["norm_k_img"]
+        plain = {"norm_q": "norm_q.weight", "norm_k": "norm_k.weight", "w_o": "to_out.weight", "b_o": "to_out.bias",
+                 "norm2_w": "self_attn_residual_norm.norm.weight", "norm2_b": "self_attn_residual_norm.norm.bias",
+                 "w_q2": "attn2.to_q.weight", "b_q2": "attn2.to_q.bias", "norm_q2": "attn2.norm_q.weight",
+                 "norm_k2": "attn2.norm_k.weight", "w_o2": "attn2.to_out.weight", "b_o2": "attn2.to_out.bias",
+                 "w_1": "ffn.fc_in.weight", "b_1": "ffn.fc_in.bias", "w_2": "ffn.fc_out.weight", "b_2": "ffn.fc_out.bias",
+                 "scale_shift_table": "scale_shift_table"}
+        for src, dst in plain.items():
+            out[dst] = t[src]
+        return {prefix + k: v for k, v in out.items()}
 
 
 @dataclass
@@ -251,59 +289,99 @@ class CrossAttnCache:
 I2V_IMAGE_TOKENS = 257  # wanvideo.py:259-260: the first 257 context rows are the CLIP image tokens
 
 
+def _keep(keep: dict | None, **tensors) -> None:
+    """With `keep` (the block under grad, _WanBlockFn), record tensors the backward needs."""
+    if keep is not None:
+        keep.update(tensors)
+
+
+def _linear_kept(keep: dict | None, name: str, x, w, bias, epilogue: int, **kw) -> torch.Tensor:
+    """linear_any; with `keep`, the bf16 y the epilogue consumes is kept under `name` as well (fvb_linear_bf16_aux)."""
+    if keep is None:
+        return ops.linear_any(x, w, bias, epilogue, **kw)
+    out, keep[name] = ops.linear_aux(x, w, bias, epilogue, **kw)
+    return out
+
+
+def _attention_kept(keep: dict | None, name: str, q, k, v, softmax_scale: float) -> torch.Tensor:
+    """ops.attention; with `keep`, its log-sum-exp is kept under `name`."""
+    if keep is None:
+        return ops.attention(q, k, v, softmax_scale=softmax_scale)
+    out, keep[name] = ops.attention(q, k, v, softmax_scale=softmax_scale, return_lse=True)
+    return out
+
+
 def cross_attention(n2: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, cfg: WanDiTConfig,
-                    xcache: CrossAttnCache | None = None) -> torch.Tensor:
+                    xcache: CrossAttnCache | None = None, keep: dict | None = None) -> torch.Tensor:
     """WanT2VCrossAttention.forward (wanvideo.py:188-222), or WanI2VCrossAttention.forward (:225-280) when the block
     carries add_k_proj / add_v_proj: text attention + image-token attention, summed in bf16. Returns [S, D] (pre to_out).
-    With `xcache`, the text K/V are computed on the first call and reused afterwards."""
+    With `xcache`, the text K/V are computed on the first call and reused afterwards. `keep`: see _keep."""
     S, D = n2.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
     hd = lambda t: t.unflatten(1, (H, d)).unsqueeze(0)
     q2 = ops.linear_any(n2, blk.w_q2, blk.b_q2)
+    _keep(keep, q2_pre=q2.clone() if keep is not None else None)
     ops.rmsnorm_rope_(q2, blk.norm_q2, head_dim=d, eps=cfg.eps)
     img = None
     if blk.w_kv_img is not None:
         ctx_img, ctx = ctx[:I2V_IMAGE_TOKENS], ctx[I2V_IMAGE_TOKENS:]
         kvi = ops.linear_any(ctx_img.contiguous(), blk.w_kv_img, blk.b_kv_img)
+        _keep(keep, ki_pre=kvi[:, :D].clone() if keep is not None else None)
         ops.rmsnorm_rope_(kvi[:, :D], blk.norm_k_img, head_dim=d, eps=cfg.eps)
-        img = ops.attention(hd(q2), hd(kvi[:, :D]), hd(kvi[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
+        img = _attention_kept(keep, "lse_i", hd(q2), hd(kvi[:, :D]), hd(kvi[:, D:]), d ** -0.5).reshape(S, D)
+        _keep(keep, kvi=kvi, img=img)
         if ctx.shape[0] == 0:
+            if keep is not None:
+                raise ops.FvbError("the I2V block backward needs text tokens after the 257 image tokens")
             return img  # zeros_like(q) + img_x
     if xcache is not None and xcache.kv is not None:
         kv2 = xcache.kv
     else:
         kv2 = ops.linear_any(ctx.contiguous(), blk.w_kv2, blk.b_kv2)  # [L, 2D]
+        _keep(keep, k2_pre=kv2[:, :D].clone() if keep is not None else None)
         ops.rmsnorm_rope_(kv2[:, :D], blk.norm_k2, head_dim=d, eps=cfg.eps)
         if xcache is not None:
             xcache.kv = kv2
-    a2 = ops.attention(hd(q2), hd(kv2[:, :D]), hd(kv2[:, D:]), softmax_scale=d ** -0.5).reshape(S, D)
+    a2 = _attention_kept(keep, "lse2", hd(q2), hd(kv2[:, :D]), hd(kv2[:, D:]), d ** -0.5).reshape(S, D)
+    _keep(keep, q2=q2, kv2=kv2, a2t=a2)
     return a2 if img is None else a2 + img  # `x = x + img_x` on bf16 tensors
 
 
 def block_tail(y: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulation, cfg: WanDiTConfig,
-               xcache: CrossAttnCache | None = None) -> torch.Tensor:
+               xcache: CrossAttnCache | None = None, keep: dict | None = None) -> torch.Tensor:
     """The block after the self-attention out-projection y (fp32 or bf16, per mod.attn_epilogue): LayerNorm(affine),
-    cross-attention, feed-forward (wanvideo.py:415-432, causal_wanvideo.py:321-340). Returns [S, D] bf16."""
+    cross-attention, feed-forward (wanvideo.py:415-432, causal_wanvideo.py:321-340). Returns [S, D] bf16. `keep`: see
+    _keep (fp32 modulation flow only)."""
     if mod.bf16:  # LayerNorm of the bf16 residual (layernorm.py:159-213)
         n2, x = ops.layernorm_modulate(y, None, None, blk.norm2_w, blk.norm2_b, round_ln=True, eps=cfg.eps), y
     else:  # LayerNorm of the fp32 residual, which also becomes the bf16 residual stream
         n2, x = ops.layernorm_modulate(y, None, None, blk.norm2_w, blk.norm2_b, eps=cfg.eps, want_hidden=True)
-    a2 = cross_attention(n2, blk, ctx, cfg, xcache)
+    a2 = cross_attention(n2, blk, ctx, cfg, xcache, keep)
     x = ops.linear_any(a2, blk.w_o2, blk.b_o2, ops.EPI_RESID_BF16, resid=x)
     n3 = ops.layernorm_modulate(x, mod.c_scale, mod.c_shift, round_ln=True, eps=cfg.eps, mod_rows=mod.rows, mod_bf16=mod.bf16)
-    f = ops.linear_any(n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
-    return ops.linear_any(f, blk.w_2, blk.b_2, mod.ffn_epilogue, resid=x, gate=mod.c_gate, gate_rows=mod.rows)
+    f = _linear_kept(keep, "h", n3, blk.w_1, blk.b_1, ops.EPI_BIAS_GELU_TANH)
+    _keep(keep, n2=n2, a2=a2, x2=x, n3=n3, f=f)
+    return _linear_kept(keep, "o3", f, blk.w_2, blk.b_2, mod.ffn_epilogue, resid=x, gate=mod.c_gate, gate_rows=mod.rows)
 
 
 def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torch.Tensor, lay: TokenLayout,
                   cfg: WanDiTConfig) -> torch.Tensor:
-    """x: [S, D] bf16 (one sample), ctx: [L, D] bf16 text states, temb6: [1, 6, D] (timestep_proj). Returns [S, D]."""
+    """x: [S, D] bf16 (one sample), ctx: [L, D] bf16 text states, temb6: [1, 6, D] (timestep_proj). Returns [S, D].
+    Differentiable (in x, ctx, temb6 and every tensor of blk.tensors()) when grad is enabled and one of them requires grad:
+    the block then runs _WanBlockFn, whose forward is this same body (block_body) and returns the same bits."""
+    if torch.is_grad_enabled() and _any_requires_grad(blk, x, ctx, temb6):
+        return _block_forward_grad(x, blk, ctx, temb6, lay, cfg)
+    return block_body(x, blk, ctx, Modulation.fp32(blk, temb6), lay, cfg)
+
+
+def block_body(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulation, lay: TokenLayout, cfg: WanDiTConfig,
+               keep: dict | None = None) -> torch.Tensor:
+    """The single-rank block: self-attention (wanvideo.py:393-415), then block_tail. `keep`: see _keep."""
     S, D = x.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
-    mod = Modulation.fp32(blk, temb6)
-    # self-attention (wanvideo.py:393-415)
     n1 = mod.norm1(x, cfg.eps)
     qkv = ops.linear_any(n1, blk.w_qkv, blk.b_qkv)  # [S, 3D or 4D]
+    _keep(keep, n1=n1, qkv=qkv, qk_pre=qkv[:, :2 * D].clone() if keep is not None else None)
     ops.rmsnorm_rope_(qkv[:, :D], blk.norm_q, qkv[:, D:2 * D], blk.norm_k, lay.cos, lay.sin, lay.rope_row, head_dim=d,
                       eps=cfg.eps)
     q = qkv[:, :D].unflatten(1, (H, d)).unsqueeze(0)
@@ -311,14 +389,166 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
     v = qkv[:, 2 * D:3 * D].unflatten(1, (H, d)).unsqueeze(0)
     if cfg.vsa:
         gate = qkv[:, 3 * D:4 * D].unflatten(1, (H, d)).unsqueeze(0)
-        a = vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=gate, block_off=lay.block_off,
-                                       row_block=lay.row_block, attn_8bit=cfg.attention_8bit)
+        if keep is None:
+            a = vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=gate, block_off=lay.block_off,
+                                           row_block=lay.row_block, attn_8bit=cfg.attention_8bit)
+        else:  # the same kernels in the same order (bit-identical), keeping what the VSA backward needs
+            vctx = _SavedCtx()
+            a = vsa._VideoSparseAttnFn.forward(vctx, q, k, v, gate, lay.vbs, lay.topk, None, lay.block_off, lay.row_block)
+            keep["vsa"] = vctx.saved_tensors
     elif cfg.attention_8bit:
         a = ops.attention_8bit(ops.quantize_attention_8bit(q, k, v), d ** -0.5)
     else:
-        a = ops.attention(q, k, v, softmax_scale=d ** -0.5)
-    y = ops.linear_any(a.reshape(S, D), blk.w_o, blk.b_o, mod.attn_epilogue, resid=x, gate=mod.gate_msa, gate_rows=mod.rows)
-    return block_tail(y, blk, ctx, mod, cfg)
+        a = _attention_kept(keep, "lse", q, k, v, d ** -0.5)
+    _keep(keep, a=a.reshape(S, D))
+    y = _linear_kept(keep, "o1", a.reshape(S, D), blk.w_o, blk.b_o, mod.attn_epilogue, resid=x, gate=mod.gate_msa,
+                     gate_rows=mod.rows)
+    _keep(keep, y=y)
+    return block_tail(y, blk, ctx, mod, cfg, keep=keep)
+
+
+# ------------------------------------------------------------------------------------------------ block backward
+def _any_requires_grad(blk: WanBlock, *inputs) -> bool:
+    # quantised weights (ops.Fp8Weight / ops.Int8Weight) are not tensors and never require grad
+    return any(getattr(t, "requires_grad", False) for t in (*inputs, *blk.tensors().values()))
+
+
+def refuse_grad(path: str, blk: WanBlock, *inputs) -> None:
+    """Raise FvbError when a block path without a backward would run under grad with something requiring grad (it would
+    otherwise return an output without a grad_fn)."""
+    if torch.is_grad_enabled() and _any_requires_grad(blk, *inputs):
+        raise ops.FvbError(f"{path} has no backward: run it under torch.no_grad(), or train the single-rank block "
+                           "(wan_dit.block_forward)")
+
+
+_BLOCK_TENSORS = ("w_qkv", "b_qkv", "norm_q", "norm_k", "w_o", "b_o", "norm2_w", "norm2_b", "w_q2", "b_q2", "w_kv2", "b_kv2",
+                  "norm_q2", "norm_k2", "w_o2", "b_o2", "w_1", "b_1", "w_2", "b_2", "w_kv_img", "b_kv_img", "norm_k_img")
+_FN_LEAD = 11  # _WanBlockFn inputs before the block tensors: x, ctx, six modulation vectors, blk, lay, cfg
+
+
+def _block_forward_grad(x, blk: WanBlock, ctx, temb6, lay: TokenLayout, cfg: WanDiTConfig) -> torch.Tensor:
+    if not blk.trainable or cfg.attention_8bit:
+        raise ops.FvbError("the Wan block backward covers bf16 linears and bf16 attention: fp8_linears, int8_weights / "
+                           "int8_activations and attention_8bit run without grad only")
+    for n in ("norm_q", "norm_k", "norm_q2", "norm_k2", "norm_k_img"):
+        t = getattr(blk, n)
+        if t is not None and t.dtype != torch.bfloat16:
+            raise ops.FvbError(f"the Wan block backward needs bf16 RMSNorm weights ({n} is {t.dtype})")
+    if cfg.vsa and vsa.SPARSE_KERNEL != "ws":
+        raise ops.FvbError("the VSA backward needs the block-list sparse kernel (FVB_VSA_KERNEL=ws)")
+    mod = Modulation.fp32(blk, temb6)  # torch ops: autograd carries the six vectors back to scale_shift_table and temb6
+    return _WanBlockFn.apply(x, ctx, mod.shift_msa, mod.scale_msa, mod.gate_msa, mod.c_shift, mod.c_scale, mod.c_gate, blk, lay,
+                             cfg, *(getattr(blk, n) for n in _BLOCK_TENSORS))
+
+
+class _SavedCtx:
+    """Stands in for an autograd ctx when _VideoSparseAttnFn runs inside _WanBlockFn (its tensors are then saved by
+    _WanBlockFn's own ctx)."""
+
+    def save_for_backward(self, *t):
+        self.saved_tensors = t
+
+
+class _WanBlockFn(torch.autograd.Function):
+    """block_forward with autograd. The forward is block_body with a `keep` dict: the same kernel calls (same bits), plus
+    storage for the backward -- the pre-norm q / k / q2 / k2 (cloned before the in-place norms), the attention LSEs, and the
+    pre-epilogue bf16 y of the fc_in / to_out / fc_out GEMMs (fvb_linear_bf16_aux). The backward is torch autograd's for the
+    reference block (DESIGN.md "Wan block backward"); weight / bias / context gradients that no input needs are skipped."""
+
+    @staticmethod
+    def forward(fctx, x, ctx, shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, blk, lay, cfg, *params):
+        keep = {}
+        mod = Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate)
+        out = block_body(x.detach(), blk, ctx.detach(), mod, lay, cfg, keep)
+        vsa_saved = keep.pop("vsa", ())
+        fctx.blk, fctx.lay, fctx.cfg = blk, lay, cfg
+        fctx.names = tuple(keep)
+        fctx.save_for_backward(x, ctx, scale_msa, gate_msa, c_scale, c_gate, *keep.values(), *vsa_saved)
+        return out
+
+    @staticmethod
+    def backward(fctx, dout):
+        x, ctx, scale_msa, gate_msa, c_scale, c_gate = fctx.saved_tensors[:6]
+        names = fctx.names
+        kp = dict(zip(names, fctx.saved_tensors[6:6 + len(names)]))
+        vsa_saved = fctx.saved_tensors[6 + len(names):]
+        blk, lay, cfg = fctx.blk, fctx.lay, fctx.cfg
+        need = lambda n: fctx.needs_input_grad[_FN_LEAD + _BLOCK_TENSORS.index(n)]
+        S, D = x.shape
+        H, d = cfg.num_attention_heads, cfg.head_dim
+        hd = lambda t: t.unflatten(1, (H, d)).unsqueeze(0)
+        eps = cfg.eps
+        want_dctx = fctx.needs_input_grad[1]
+        g = {}
+        dout = dout.to(torch.bfloat16).contiguous()
+        # feed-forward: out = bf16(x2 + o3 * c_gate), o3 = fc_out(f), f = gelu(h), h = fc_in(n3)
+        d_o3, d_cgate, g["b_2"] = ops.resid_gate_bwd(dout, kp["o3"], c_gate, need_db=need("b_2"))
+        if need("w_2"):
+            g["w_2"] = ops.linear_bwd(kp["f"], blk.w_2, d_o3, need_dx=False)[1]
+        dh = ops.linear_dgrad_gelu(d_o3, blk.w_2, kp["h"])
+        dn3, g["w_1"], g["b_1"] = ops.linear_bwd(kp["n3"], blk.w_1, dh, need_dw=need("w_1"), need_db=need("b_1"))
+        dx2, d_cscale, d_cshift = ops.layernorm_modulate_bwd(kp["x2"], dn3, scale=c_scale, round_ln=True, gin=dout, eps=eps)
+        # cross-attention: x2 = bf16(xb + to_out2(a2)), a2 = a2t (+ img)
+        da2, g["w_o2"], g["b_o2"] = ops.linear_bwd(kp["a2"], blk.w_o2, dx2, need_dw=need("w_o2"), need_db=need("b_o2"))
+        q2, kv2 = kp["q2"], kp["kv2"]
+        dq2, dk2, dv2 = ops.attention_bwd(hd(q2), hd(kv2[:, :D]), hd(kv2[:, D:]), hd(kp["a2t"]), kp["lse2"], hd(da2),
+                                          softmax_scale=d ** -0.5)
+        dq2 = dq2.view(S, D)
+        ctx_txt = ctx[I2V_IMAGE_TOKENS:] if blk.w_kv_img is not None else ctx
+        dctx_txt = dctx_img = None
+        if want_dctx or need("w_kv2") or need("b_kv2") or need("norm_k2"):
+            dkv2 = torch.empty_like(kv2)
+            dk2_pre, g["norm_k2"] = ops.rmsnorm_bwd(kp["k2_pre"], blk.norm_k2, dk2.view(-1, D), eps=eps,
+                                                    want_dw=need("norm_k2"))
+            dkv2[:, :D].copy_(dk2_pre)
+            dkv2[:, D:].copy_(dv2.view(-1, D))
+            dctx_txt, g["w_kv2"], g["b_kv2"] = ops.linear_bwd(ctx_txt.contiguous(), blk.w_kv2, dkv2, need_dx=want_dctx,
+                                                               need_dw=need("w_kv2"), need_db=need("b_kv2"))
+        if blk.w_kv_img is not None:
+            kvi = kp["kvi"]
+            dq2i, dki, dvi = ops.attention_bwd(hd(q2), hd(kvi[:, :D]), hd(kvi[:, D:]), hd(kp["img"]), kp["lse_i"], hd(da2),
+                                               softmax_scale=d ** -0.5)
+            dq2 = dq2 + dq2i.view(S, D)
+            if want_dctx or need("w_kv_img") or need("b_kv_img") or need("norm_k_img"):
+                dkvi = torch.empty_like(kvi)
+                dki_pre, g["norm_k_img"] = ops.rmsnorm_bwd(kp["ki_pre"], blk.norm_k_img, dki.view(-1, D), eps=eps,
+                                                           want_dw=need("norm_k_img"))
+                dkvi[:, :D].copy_(dki_pre)
+                dkvi[:, D:].copy_(dvi.view(-1, D))
+                dctx_img, g["w_kv_img"], g["b_kv_img"] = ops.linear_bwd(
+                    ctx[:I2V_IMAGE_TOKENS].contiguous(), blk.w_kv_img, dkvi, need_dx=want_dctx, need_dw=need("w_kv_img"),
+                    need_db=need("b_kv_img"))
+        dctx = None
+        if want_dctx:
+            dctx = dctx_txt if dctx_img is None else torch.cat([dctx_img, dctx_txt], 0)
+        dq2_pre, g["norm_q2"] = ops.rmsnorm_bwd(kp["q2_pre"], blk.norm_q2, dq2, eps=eps, want_dw=need("norm_q2"))
+        dn2, g["w_q2"], g["b_q2"] = ops.linear_bwd(kp["n2"], blk.w_q2, dq2_pre, need_dw=need("w_q2"), need_db=need("b_q2"))
+        # norm2 of the fp32 residual y (n2 = bf16(LN(y) w + b)); xb = bf16(y) carries dx2 into dy as well
+        dy, g["norm2_w"], g["norm2_b"] = ops.layernorm_modulate_bwd(kp["y"], dn2, weight=blk.norm2_w, gin=dx2, eps=eps)
+        # self-attention out-projection: y = x + o1 * gate_msa
+        d_o1, d_gate_msa, g["b_o"] = ops.resid_gate_bwd(dy, kp["o1"], gate_msa, need_db=need("b_o"))
+        da, g["w_o"], _ = ops.linear_bwd(kp["a"], blk.w_o, d_o1, need_dw=need("w_o"))
+        qkv = kp["qkv"]
+        dqkv = torch.empty_like(qkv)
+        if cfg.vsa:
+            vctx = _SavedCtx()
+            vctx.saved_tensors = vsa_saved
+            vctx.needs_input_grad = (True, True, True, True)
+            dq, dk, dv, dgate = vsa._VideoSparseAttnFn.backward(vctx, hd(da))[:4]
+            dqkv[:, 3 * D:].copy_(dgate.view(S, D))
+        else:
+            q, k, v = hd(qkv[:, :D]), hd(qkv[:, D:2 * D]), hd(qkv[:, 2 * D:3 * D])
+            dq, dk, dv = ops.attention_bwd(q, k, v, hd(kp["a"]), kp["lse"], hd(da), softmax_scale=d ** -0.5)
+        dqkv[:, 2 * D:3 * D].copy_(dv.reshape(S, D))
+        qk_pre = kp["qk_pre"]
+        g["norm_q"], g["norm_k"] = ops.rmsnorm_rope_bwd(qk_pre[:, :D], blk.norm_q, dq.reshape(S, D), dqkv[:, :D],
+                                                        qk_pre[:, D:], blk.norm_k, dk.reshape(S, D), dqkv[:, D:2 * D],
+                                                        lay.cos, lay.sin, lay.rope_row, head_dim=d, eps=eps,
+                                                        want_dw=need("norm_q") or need("norm_k"))
+        dn1, g["w_qkv"], g["b_qkv"] = ops.linear_bwd(kp["n1"], blk.w_qkv, dqkv, need_dw=need("w_qkv"), need_db=need("b_qkv"))
+        dx, d_scale_msa, d_shift_msa = ops.layernorm_modulate_bwd(x, dn1, scale=scale_msa, gin=dy, eps=eps)
+        return (dx, dctx, d_shift_msa, d_scale_msa, d_gate_msa, d_cshift, d_cscale, d_cgate, None, None, None,
+                *(g.get(n) if need(n) else None for n in _BLOCK_TENSORS))
 
 
 class WanDiT:

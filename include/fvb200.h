@@ -103,6 +103,34 @@ int64_t fvb_bias_grad_bf16_workspace_bytes(int M, int N);
 int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float* workspace, int64_t workspace_bytes, int M, int N,
                        void* stream);
 
+/* Pieces of the Wan block backward that live in GEMM epilogues (bf16 operands, the arguments of fvb_linear_bf16):
+ * fvb_linear_bf16_aux: fvb_linear_bf16 that also stores the bf16 y = bf16(acc + bias) its epilogue consumes to
+ *   aux[m * ldaux + n] (ldaux a multiple of 8, >= N; N a multiple of 8). Epilogues FVB_EPI_BIAS_GELU_TANH (aux = the fc_in
+ *   output before the GELU), FVB_EPI_RESID_GATE_F32 and FVB_EPI_RESID_GATE_BF16 (aux = the projection before the gate
+ *   multiply). `out` gets the same bits as fvb_linear_bf16, and aux the same bits as fvb_linear_bf16 with FVB_EPI_BIAS.
+ * fvb_linear_dgrad_gelu_bf16: fvb_linear_dgrad_bf16 with the GELU(tanh) backward in its epilogue, for y = w2 . gelu(h):
+ *   dh[m, k] = bf16(float(bf16(sum_n dy[m, n] * w[n, k])) * gelu_tanh'(h[m, k]))     h bf16 [M, K] (ldh a multiple of 8)
+ *   gelu_tanh'(h) = 0.5 (1 + t) + 0.5 h (1 - t^2) sqrt(2/pi) (1 + 3 * 0.044715 h^2), t = tanh(sqrt(2/pi) (h + 0.044715 h^3)),
+ *   t evaluated as FVB_EPI_BIAS_GELU_TANH evaluates it. Torch's rounding: bf16 F.linear dgrad, then bf16 gelu_backward. */
+int fvb_linear_bf16_aux(const void* x, int64_t ldx, const void* w, int64_t ldw, const void* bias, void* out, int64_t ldo,
+                        const void* resid, int64_t ldr, const float* gate, int gate_rows, int64_t gate_stride, void* aux,
+                        int64_t ldaux, int M, int N, int K, int epilogue, void* stream);
+int fvb_linear_dgrad_gelu_bf16(const void* dy, int64_t lddy, const void* w, int64_t ldw, const void* h, int64_t ldh, void* dh,
+                               int64_t lddh, int M, int N, int K, void* stream);
+
+/* Backward of the gated residual out = resid + y * gate[n] (FVB_EPI_RESID_GATE_F32 / _BF16) given dout [M, N] (fp32 when
+ * dout_is_f32, else bf16) and the saved bf16 y [M, N] (fvb_linear_bf16_aux's aux); gate fp32 [N]:
+ *   dy[m, n] = bf16(dout * gate[n])                 bf16 [M, N] (lddy)
+ *   d_gate[n] = sum_m dout * y                      fp32 [N]
+ *   db[n] = bf16(sum_m float(dy[m, n]))             bf16 [N], the projection's bias gradient (db NULL: skipped)
+ * The residual's gradient is dout itself (nothing is written for it). N a multiple of 8; strides keep rows 16-byte aligned.
+ * Column sums as in fvb_bias_grad_bf16: min(M, 256) fixed row sets summed in row order, partials added in row-set order;
+ * no atomics. workspace: fvb_resid_gate_bwd_workspace_bytes(M, N) bytes, 16-byte aligned. */
+int64_t fvb_resid_gate_bwd_workspace_bytes(int M, int N);
+int fvb_resid_gate_bwd(const void* dout, int dout_is_f32, int64_t lddout, const void* y, int64_t ldy, const float* gate, void* dy,
+                       int64_t lddy, float* d_gate, void* db, float* workspace, int64_t workspace_bytes, int M, int N,
+                       void* stream);
+
 /* --------------------------------------------------------------------------------------------
  * FP8 (e4m3) linear layers: row-quantised activations x per-output-channel-quantised weights
  * Stands behind FastVideo's FP8 linear (fastvideo/layers/fp8linear.py, fastvideo/layers/quantization/) with this
@@ -252,6 +280,35 @@ int fvb_rmsnorm_rope_scatter(const void* x0, const void* w0, int64_t ld0, const 
 int64_t fvb_rmsnorm_bwd_workspace_bytes(int M, int D);
 int fvb_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const void* dy, int64_t lddy, void* dx, int64_t lddx, void* dw,
                     float* workspace, int64_t workspace_bytes, int M, int D, float eps, void* stream);
+
+/* Backward of fvb_rmsnorm_rope with RoPE, for x0 (and x1: q and k in one launch, blockIdx.y selects), bf16 weights only;
+ * cos / sin fp32 [S_pos, head_dim] and rope_row as in the forward. dy is the gradient of the rotated output. Per pair
+ * (2i, 2i+1) of each row, fp32, the forward's rotation transposed:
+ *   dn[2i]   = bf16(dy[2i] * cos[2i] + dy[2i+1] * sin[2i+1])
+ *   dn[2i+1] = bf16(dy[2i+1] * cos[2i+1] - dy[2i] * sin[2i])
+ * then fvb_rmsnorm_bwd's arithmetic with dn in place of dy (dx, and dw0 / dw1 with their own partials when dw0 != NULL).
+ * workspace: fvb_rmsnorm_rope_bwd_workspace_bytes(M, D) bytes (two tensors' partials). */
+int64_t fvb_rmsnorm_rope_bwd_workspace_bytes(int M, int D);
+int fvb_rmsnorm_rope_bwd(const void* x0, int64_t ldx0, const void* w0, const void* dy0, int64_t lddy0, void* dx0, int64_t lddx0,
+                         void* dw0, const void* x1, int64_t ldx1, const void* w1, const void* dy1, int64_t lddy1, void* dx1,
+                         int64_t lddx1, void* dw1, const float* cos_t, const float* sin_t, const int32_t* rope_row,
+                         float* workspace, int64_t workspace_bytes, int M, int D, int head_dim, float eps, void* stream);
+
+/* Backward of fvb_layernorm_modulate's single-row-group forms: n = bf16(t * gain[c] + offset[c]), t = LN(x) =
+ * (x - mean) * rstd (fp32, biased variance, recomputed from x), t rounded to bf16 first with round_ln. gain is (1 + scale)
+ * with gain_is_scale (modulation: offset = shift) or the affine weight w (offset = the affine bias). x [M, D] bf16, or fp32
+ * with x_is_f32; dn bf16 [M, D]; round_ln only with gain_is_scale. Per row, fp32:
+ *   dt = dn * gain,  dx = rstd * ((dt - mean_c(dt)) - t~ * mean_c(dt * t~))  (t~ = the unrounded t)  [+ gin]
+ *   dx: fp32 when x is fp32, else bf16 (one rounding after the optional incoming gradient gin, fp32 or bf16 per gin_is_f32,
+ *   is added: the residual stream's two gradient contributions meet here)
+ *   d_gain[c] = sum_m dn * t (t as used in the forward, bf16 with round_ln), d_offset[c] = sum_m dn    (fp32 [D])
+ * Column sums as in fvb_rmsnorm_bwd (min(M, 528) CTAs, partials added in CTA order). D a multiple of 8, <= 8192; strides
+ * multiples of 8. workspace: fvb_layernorm_modulate_bwd_workspace_bytes(M, D) bytes, 16-byte aligned. */
+int64_t fvb_layernorm_modulate_bwd_workspace_bytes(int M, int D);
+int fvb_layernorm_modulate_bwd(const void* x, int x_is_f32, int64_t ldx, const void* dn, int64_t lddn, const float* gain,
+                               int gain_is_scale, int round_ln, const void* gin, int gin_is_f32, int64_t ldgin, void* dx,
+                               int64_t lddx, float* d_gain, float* d_offset, float* workspace, int64_t workspace_bytes, int M,
+                               int D, float eps, void* stream);
 
 /* --------------------------------------------------------------------------------------------
  * Attention forward, head_dim 128, bf16, fp32 softmax. Dense or block-list (VSA / STA) keys.
