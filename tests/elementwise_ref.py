@@ -1,0 +1,424 @@
+"""Element-by-element references for the wgmma GEMM (csrc/gemm_sm90.cu) and the bf16 attention forward (csrc/attn_sm90.cu).
+
+Two kinds of check, for two kinds of bug.
+
+(a) Exact-arithmetic inputs, compared bit for bit (data-movement bugs).
+    Operands on the grid x = a * 2^-4, |a| <= 15 (grid_bf16): every product is a multiple of 2^-8 below 2^8 in size, so
+    every partial sum of K <= 13824 products is an integer number of 2^-8 quanta below 225 * 13824 < 2^22 quanta. fp32 holds
+    such sums exactly, in any summation order, on any adder that keeps 24 bits. The bias lives on the same grid, so
+    acc + bias is exact too. The kernel's output is then fully determined by the rounding points of include/fvb200.h,
+    which epilogue_ref replays with separate torch fp32 ops (torch's fp32 elementwise ops are IEEE round-to-nearest, like
+    the kernel's __fmul_rn / __fadd_rn / __fdiv_rn; divisions use a tensor divisor, since torch turns a scalar divisor
+    into a reciprocal multiply).
+    GELU(tanh) uses ex2.approx and __fdividef, so its outputs are bounded instead (gelu_grid_bound): with
+    t = 1 - q, q = 2 / (e + 1) in (0, 2), the kernel's t differs from tanh by at most 2^-24 (the subtraction) plus
+    |q| * (2 ulp of __fdividef + 2^-22 of ex2.approx + the rounding of its argument), below 2^-20 in total; gelu =
+    0.5 y (1 + t) turns that into an absolute 2^-21 |y|, which dominates when 1 + t cancels (y below about -4: a purely
+    relative bound fails there). The products and the final bf16 store add one bf16 ulp of the result.
+
+(b) fp64 element bounds on ordinary random inputs (numerical bugs).
+    Per output element e = sum_k x w (fp64) and A = sum_k |x w|. The tensor cores add the 16 exact products of each k16
+    step to the fp32 accumulator in one operation: at most one truncation of the result (relative 2^-23) plus the
+    alignment of the 17 addends (another 2^-23 of their magnitude sum), i.e. 2^-22 * A per step. With n = ceil(K / 16)
+    steps (the k-block chains of one tile run in k order) |acc - e| <= c A, c = n * 2^-22 (acc_coeff). The epilogue then
+    adds the bias (2^-24 relative) and rounds y to bf16 (half a bf16 ulp of y); epilogue_bound carries |y - e'| through
+    each epilogue with its derivative (|gate|, 1, 1 / div, |gelu'| <= 1.13) and adds each of its own roundings.
+
+Attention constructions (tie_attention_ref), exact for the bf16 kernel's online softmax:
+    Logits are exact small integers (q, k on integer grids), so every logit equals the kernel's fp32 x = fl(s * scale_log2)
+    bit for bit. If every visible key's x is either the row maximum m or at least 150 below it, the keys at m get p = 1
+    (ex2(0)), the rest p = 0 (ex2 underflows), and with v on the grid o = bf16(sum_T v * (1 / |T|)) exactly (IEEE
+    division, no fast-math); LSE = m + log2f(|T|), within one fp32 ulp.
+    uniform: q = 0, every visible key ties (|T| = visible count): any masked key counted or visible key dropped moves o and
+             LSE.
+    one-hot: every key of a (b, h) has its own code, a one-hot slot channel and a one-hot group channel of magnitude 64
+             (onehot_qk); each q row copies one visible target key. The target's logit is 8192, every other key's at most
+             4096, so one key per row sits 4096 * scale * log2 e (>= 150 for scale >= 0.026) above the rest, for any
+             number of visible keys up to 4096: o is that key's v row and LSE its logit. Codes and targets differ per
+             (b, h, row), so reading the wrong head, batch, key block or row offset gives another row.
+    Random inputs use attention_bound: the fp32 logit error (c * sum |q k| from the QK^T chain, plus 3 roundings of
+    x) is amplified through exp2 into a relative error rho of each p; P's bf16 rounding (relative 2^-8) and the P V chain
+    add relative errors on each p |v|; the output rounds once more (half a bf16 ulp).
+"""
+import math
+
+import torch
+
+U32 = 2.0 ** -24  # fp32 unit roundoff (round to nearest)
+TC_STEP = 2.0 ** -22  # one k16 tensor-core accumulation step, relative to the magnitude sum (see (b))
+LOG2E = 1.4426950408889634
+
+EPI_BIAS, EPI_GELU, EPI_GATE_F32, EPI_GATE_BF16, EPI_RESID_BF16, EPI_DIV, EPI_SCALE_F32, EPI_GATE_BF16R = 0, 1, 2, 3, 4, 5, 6, 7
+
+# per kernel family: the largest error / bound ratio seen on random inputs, and the outputs compared bit for bit
+MAX_RATIO: dict = {}
+BIT_EXACT: dict = {}
+
+
+def ulp_bf16(v):
+    """One bf16 ulp at each value of v (float64): 2^(exponent - 7)."""
+    a = v.double().abs().clamp_min(2.0 ** -126)
+    return torch.exp2(torch.floor(torch.log2(a)) - 7)
+
+
+def half_ulp_bf16(v):
+    return ulp_bf16(v) * 0.5
+
+
+def ulp_f32(v):
+    a = v.double().abs().clamp_min(2.0 ** -126)
+    return torch.exp2(torch.floor(torch.log2(a)) - 23)
+
+
+def f32(x: float) -> float:
+    """x rounded to fp32 (what a float argument of the C ABI holds)."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def grid_bf16(shape, gen, device, lim=15, scale=2.0 ** -4):
+    """bf16 values a * scale with integer |a| <= lim."""
+    a = torch.randint(-lim, lim + 1, tuple(shape), generator=gen, device=device)
+    return (a.to(torch.float32) * scale).bfloat16()
+
+
+def rand_bf16(shape, gen, device, scale=1.0):
+    return (torch.randn(tuple(shape), generator=gen, device=device) * scale).bfloat16()
+
+
+def acc_coeff(K: int) -> float:
+    return math.ceil(K / 16) * TC_STEP
+
+
+def exact_gemm(a, b):
+    """e = a @ b^T and A = |a| @ |b|^T in fp64 (a [.., M, K], b [.., N, K])."""
+    a64, b64 = a.double(), b.double()
+    return a64 @ b64.transpose(-1, -2), a64.abs() @ b64.abs().transpose(-1, -2)
+
+
+def print_summary(config) -> None:
+    """Print the per-family largest error / bound ratio and bit-exact counts, past pytest's output capture."""
+    lines = ["", "elementwise checks so far (error / bound ratios on random inputs unless the family says grid inputs):"]
+    lines += [f"  {k}: largest error / bound {v:.3e}" for k, v in sorted(MAX_RATIO.items())]
+    lines += [f"  {k}: {v} outputs compared bit for bit" for k, v in sorted(BIT_EXACT.items())]
+    cap = config.pluginmanager.getplugin("capturemanager")
+    if cap is None:
+        print("\n".join(lines))
+        return
+    with cap.global_and_fixture_disabled():
+        print("\n".join(lines), flush=True)
+
+
+def note_exact(family: str, n: int) -> None:
+    BIT_EXACT[family] = BIT_EXACT.get(family, 0) + int(n)
+
+
+def note_ratio(family: str, r: float) -> None:
+    MAX_RATIO[family] = max(MAX_RATIO.get(family, 0.0), r)
+
+
+# ------------------------------------------------------------------------------------------------ (a) exact references
+def epilogue_ref(acc, epi, bias=None, resid=None, gate=None, div=None, scale=None):
+    """The kernel's epilogue on an exact fp32 accumulator, rounding for rounding (include/fvb200.h). gate: fp32, already
+    expanded to [M, N] (or [N]) by the caller's row grouping."""
+    acc = acc.float()
+    if epi == EPI_SCALE_F32:
+        return acc * torch.full_like(acc, f32(scale))
+    y32 = acc if bias is None else acc + bias.float()
+    y = y32.bfloat16().float()
+    if epi == EPI_BIAS:
+        return y.bfloat16()
+    if epi == EPI_DIV:
+        return (y / torch.full_like(y, f32(div))).bfloat16()
+    r = resid.float()
+    if epi == EPI_RESID_BF16:
+        return (r + y).bfloat16()
+    yg = y * gate
+    if epi == EPI_GATE_F32:
+        return r + yg
+    if epi == EPI_GATE_BF16:
+        return (r + yg).bfloat16()
+    if epi == EPI_GATE_BF16R:
+        return (r + yg.bfloat16().float()).bfloat16()
+    raise ValueError(epi)
+
+
+def gelu64(y):
+    y = y.double()
+    return 0.5 * y * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (y + 0.044715 * y ** 3)))
+
+
+def gelu_grad64(h):
+    h = h.double()
+    k0 = math.sqrt(2.0 / math.pi)
+    t = torch.tanh(k0 * (h + 0.044715 * h ** 3))
+    return 0.5 * (1.0 + t) + 0.5 * h * (1.0 - t * t) * k0 * (1.0 + 3.0 * 0.044715 * h * h)
+
+
+def gelu_grid_bound(y):
+    """|kernel gelu_tanh(y) stored as bf16 - gelu(y)| for an exact y (module docstring (a))."""
+    ref = gelu64(y)
+    return ref, ulp_bf16(ref) + 2.0 ** -21 * y.double().abs()
+
+
+def gelu_grad_err(h):
+    """|kernel gelu_tanh'(h) - gelu'(h)|: t's absolute error (< 2^-20) enters 0.5 (1 + t) with 0.5 and 0.5 h (1 - t^2) k0
+    (1 + 3 k1 h^2) with up to 2 |t| of that, plus the formula's own ~10 fp32 roundings of terms below 1 + |h| (1 + 0.134 h^2)
+    in size: 2^-19 (1 + |h| (1 + 0.134 h^2)) covers both."""
+    h = h.double().abs()
+    return 2.0 ** -19 * (1.0 + h * (1.0 + 0.134 * h * h))
+
+
+# ------------------------------------------------------------------------------------------------ (b) fp64 bounds
+def epilogue_bound(e, A, K, epi, bias=None, resid=None, gate=None, div=None, scale=None):
+    """(reference in fp64, bound) for one epilogue on random inputs: e, A from exact_gemm, gate fp32 expanded to [M, N]."""
+    c = acc_coeff(K)
+    if epi == EPI_SCALE_F32:
+        s = f32(scale)
+        ref = e * s
+        return ref, abs(s) * c * A + U32 * ref.abs() * 2 + 1e-38
+    s = e if bias is None else e + bias.double()
+    dacc = c * (A if bias is None else A + bias.double().abs()) + (0 if bias is None else U32 * s.abs())
+    ymag = (s.abs() + dacc) * (1 + 2.0 ** -8)
+    dy = dacc + half_ulp_bf16(ymag)  # |y - s|, y = bf16(acc + bias)
+    if epi == EPI_BIAS:
+        return s, dy
+    if epi == EPI_GELU:
+        ref = gelu64(s)
+        return ref, 1.13 * dy + 2.0 ** -21 * ymag + ulp_bf16(ref.abs() + 1.13 * dy)
+    if epi == EPI_DIV:
+        d = f32(div)
+        ref = s / d
+        mag = ymag / abs(d)
+        return ref, dy / abs(d) + U32 * mag + half_ulp_bf16(mag)
+    r = resid.double()
+    if epi == EPI_RESID_BF16:
+        ref = r + s
+        mag = r.abs() + ymag
+        return ref, dy + U32 * mag + half_ulp_bf16(mag)
+    g = gate.double()
+    ref = r + s * g
+    ygmag = ymag * g.abs()
+    b = g.abs() * dy + U32 * ygmag
+    if epi == EPI_GATE_BF16R:
+        b = b + half_ulp_bf16(ygmag)
+    mag = r.abs() + ygmag + b
+    b = b + U32 * mag
+    if epi in (EPI_GATE_BF16, EPI_GATE_BF16R):
+        b = b + half_ulp_bf16(mag)
+    return ref, b
+
+
+def dgrad_gelu_bound(e, A, K, h):
+    """fvb_linear_dgrad_gelu_bf16 on random inputs: dh = bf16(bf16(acc) * gelu'(h)), e / A of the dgrad product."""
+    c = acc_coeff(K)
+    g = gelu_grad64(h)
+    dacc = c * A
+    dmag = (e.abs() + dacc) * (1 + 2.0 ** -8)
+    dd = dacc + half_ulp_bf16(dmag)
+    ref = e * g
+    b = g.abs() * dd + dmag * gelu_grad_err(h)
+    mag = ref.abs() + b
+    return ref, b + U32 * mag + half_ulp_bf16(mag)
+
+
+# ------------------------------------------------------------------------------------------------ checkers
+def gemm_coords(idx, BN, BM=128):
+    """Output element (row, col) -> (m tile, n tile, consumer warpgroup, 8-column group, column pair)."""
+    r, c = int(idx[0]), int(idx[1])
+    return dict(row=r, col=c, m_tile=r // BM, n_tile=c // BN, warpgroup=(r % BM) // 64, col_group=(c % BN) // 8,
+                col_pair=(c % 8) // 2)
+
+
+def _describe(bad, where, limit=8):
+    idx = bad.nonzero()
+    lines = [f"{idx.shape[0]} elements differ"]
+    for i in range(min(limit, idx.shape[0])):
+        lines.append(str(where(idx[i].tolist()) if where else idx[i].tolist()))
+    return "; ".join(lines)
+
+
+def assert_exact(got, ref, name, where=None, family=None):
+    """Bit-for-bit equality (NaN-free tensors)."""
+    assert got.shape == ref.shape and got.dtype == ref.dtype, f"{name}: {got.shape}/{got.dtype} vs {ref.shape}/{ref.dtype}"
+    bad = got != ref
+    assert not bool(bad.any()), f"{name}: not bit-exact: " + _describe(bad, where)
+    if family:
+        note_exact(family, got.numel())
+
+
+def assert_within(got, ref, bound, name, where=None, family=None):
+    """|got - ref| <= bound element by element (fp64); returns the largest ratio error / bound."""
+    err = (got.double() - ref.double()).abs()
+    bound = bound.double().expand_as(err)
+    bad = ~(err <= bound)
+    assert not bool(bad.any()), f"{name}: outside the element bound: " + _describe(bad, where)
+    r = float((err / bound.clamp_min(1e-300)).max()) if err.numel() else 0.0
+    if family:
+        note_ratio(family, r)
+    return r
+
+
+# ------------------------------------------------------------------------------------------------ sentinel buffers
+_INT_VIEW = {torch.bfloat16: torch.int16, torch.float16: torch.int16, torch.float32: torch.int32, torch.int32: torch.int32,
+             torch.int64: torch.int64}
+
+
+class Guarded:
+    """A buffer of random bytes; a kernel writes into views of it (view()), and assert_untouched() checks that every
+    element outside the registered regions still holds its original bits."""
+
+    def __init__(self, shape, dtype, device, seed=0):
+        self.buf = torch.empty(tuple(shape), dtype=dtype, device=device)
+        g = torch.Generator(device=device).manual_seed(seed)
+        raw = torch.randint(-2 ** 15, 2 ** 15, (self.buf.numel() * self.buf.element_size() // 2,), generator=g,
+                            device=device, dtype=torch.int32).to(torch.int16)
+        self.buf.view(-1).view(torch.int16).copy_(raw)
+        if dtype.is_floating_point:  # keep the pattern finite, so views that a kernel also reads stay usable
+            iv = self.buf.view(_INT_VIEW[dtype])
+            bad = ~torch.isfinite(self.buf)
+            iv[bad] = iv[bad] & ~(1 << (14 if dtype == torch.bfloat16 else 30))
+        self.before = self.buf.clone()
+        self.mask = torch.zeros(tuple(shape), dtype=torch.bool, device=device)
+
+    def region(self, view):
+        """Mark the elements of `view` (a view of buf) as the kernel's to write; returns view."""
+        assert view.untyped_storage().data_ptr() == self.buf.untyped_storage().data_ptr()
+        torch.as_strided(self.mask, view.shape, view.stride(), view.storage_offset() - self.buf.storage_offset()).fill_(True)
+        return view
+
+    def changed(self):
+        it = _INT_VIEW[self.buf.dtype]
+        return (self.buf.view(it) != self.before.view(it)) & ~self.mask
+
+    def assert_untouched(self, name):
+        bad = self.changed()
+        assert not bool(bad.any()), f"{name}: written outside its output: " + _describe(bad, None)
+
+
+# ------------------------------------------------------------------------------------------------ attention
+def block_of_rows(S, off, length, device):
+    """int64 [S]: the block each row belongs to as a valid row (-1: none). Block i covers rows [off[i], off[i] + length[i])."""
+    blk = torch.full((S,), -1, dtype=torch.int64, device=device)
+    for i, (o, n) in enumerate(zip(off, length)):
+        if n > 0:
+            blk[o:o + n] = i
+    return blk
+
+
+def visible_mask(B, H, Sq, Skv, device, q_block=None, kv_block=None, select=None):
+    """bool [B, H, Sq, Skv]. Dense (select None): every key < Skv. Block modes: q_block [Sq] / kv_block [Skv] from
+    block_of_rows, select bool [B or 1, H or 1, nqb, nkb]: row i sees key j when both are valid rows of blocks and the
+    row's block selects the key's."""
+    if select is None:
+        return torch.ones(B, H, Sq, Skv, dtype=torch.bool, device=device)
+    sel = select.expand(B, H, *select.shape[2:])
+    qi, kj = q_block.clamp_min(0), kv_block.clamp_min(0)
+    m = sel[:, :, qi][:, :, :, kj]
+    return m & (q_block >= 0)[:, None] & (kv_block >= 0)[None, :]
+
+
+def scale_log2_f32(softmax_scale: float) -> float:
+    """The kernel's fp32 softmax_scale * log2 e (computed in fp32 from the fp32 argument)."""
+    return float(torch.tensor(f32(softmax_scale), dtype=torch.float32) * torch.tensor(LOG2E, dtype=torch.float32))
+
+
+def tie_attention_ref(q, k, v, visible, softmax_scale):
+    """Exact output of the tie constructions (module docstring). q [B, Sq, H, 128], k / v [B, Skv, H, 128] (BSHD views),
+    visible [B, H, Sq, Skv]. Returns o bf16 [B, Sq, H, 128] (zeros for rows without keys), lse fp32 [B, H, Sq] (-inf there),
+    and the tie counts [B, H, Sq]."""
+    qh, kh, vh = (t.permute(0, 2, 1, 3).double() for t in (q, k, v))
+    s = qh @ kh.transpose(-1, -2)  # exact: integer products of small integers
+    assert bool((s == s.round()).all()), "tie construction needs integer logits"
+    x = (s.float() * torch.tensor(scale_log2_f32(softmax_scale), dtype=torch.float32, device=s.device))
+    x = x.masked_fill(~visible, float("-inf"))
+    m = x.amax(-1, keepdim=True)
+    tie = visible & (x == m)
+    gap_ok = (~visible | tie | (x.double() <= m.double() - 150)).all()
+    assert bool(gap_ok), "tie construction: a visible non-maximal logit is within 150 of the maximum"
+    cnt = tie.sum(-1).float()
+    ssum = (tie.double() @ vh).float()  # exact on the grid
+    assert bool(((tie.double() @ vh).float().double() == tie.double() @ vh).all())
+    inv = torch.ones_like(cnt) / cnt.clamp_min(1)
+    o = (ssum * inv[..., None]).bfloat16().masked_fill((cnt == 0)[..., None], 0)
+    lse = (m.squeeze(-1) + torch.log2(cnt.double()).float()).masked_fill(cnt == 0, float("-inf"))
+    return o.permute(0, 2, 1, 3), lse, cnt
+
+
+def assert_lse_tie(lse, ref, cnt, name, family=None):
+    """LSE of a tie construction: exact where one key wins, within one fp32 ulp of m + log2(count) otherwise."""
+    fin = cnt > 0
+    assert bool(torch.isinf(lse[~fin]).all() and (lse[~fin] < 0).all()), f"{name}: rows without keys need lse = -inf"
+    one = fin & (cnt == 1)
+    assert bool((lse[one] == ref[one]).all()), f"{name}: lse of one-key rows not exact: " + _describe(
+        one & (lse != ref), None)
+    err = (lse.double() - ref.double()).abs()
+    bad = fin & ~(err <= ulp_f32(ref) + ulp_f32(torch.log2(cnt.double().clamp_min(1))))
+    assert not bool(bad.any()), f"{name}: lse beyond one fp32 ulp: " + _describe(bad, None)
+    if family:
+        note_exact(family, int(fin.sum()))
+
+
+def attention_bound(q, k, v, visible, softmax_scale):
+    """fp64 reference and element bounds of o and LSE on random inputs (module docstring). Returns o_ref, o_bound
+    [B, Sq, H, 128] and lse_ref, lse_bound [B, H, Sq] (log2 domain)."""
+    qh, kh, vh = (t.permute(0, 2, 1, 3).double() for t in (q, k, v))
+    D = qh.shape[-1]
+    sl = softmax_scale * LOG2E
+    s = qh @ kh.transpose(-1, -2)
+    A = qh.abs() @ kh.abs().transpose(-1, -2)
+    x = (s * sl).masked_fill(~visible, float("-inf"))
+    dx = sl * acc_coeff(D) * A + 4 * U32 * (s * sl).abs()  # QK^T chain, then fl(scale * log2e), fl(s * scale_log2)
+    m = x.amax(-1, keepdim=True)
+    mf = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
+    P = torch.exp2(x - mf)  # 0 where masked
+    L = P.sum(-1, keepdim=True)
+    Ls = L.clamp_min(1e-300)
+    imax = x.argmax(-1, keepdim=True)
+    dxm = dx.gather(-1, imax)
+    Skv = kh.shape[2]
+    # relative error of each p: its logit and the max's, through exp2 (ln 2 per log2 unit), ex2.approx for p and the
+    # rescale factors (2^-22 each), the fp32 subtraction x - m
+    rho = math.log(2) * (dx + dxm + U32 * (x - mf).abs().nan_to_num(0, 0, 0)) + 3 * TC_STEP
+    rho = rho.masked_fill(~visible, 0)
+    o_ref = (P @ vh) / Ls
+    pv = P @ vh.abs()
+    # P V: bf16 P (2^-8), the rescaled accumulation chain (one k16 step per 16 keys), the logit errors against |v - o|
+    c_pv = acc_coeff(Skv) + 2.0 ** -8
+    dev = ((P * rho) @ vh.abs() + (P * rho).sum(-1, keepdim=True) * o_ref.abs()) / Ls
+    rho_l = (P * rho).sum(-1, keepdim=True) / Ls + Skv * U32
+    ob = (c_pv * pv / Ls + dev) / (1 - rho_l).clamp_min(0.5)
+    omag = o_ref.abs() + ob
+    ob = ob + 2 * U32 * omag + half_ulp_bf16(omag)
+    empty = (L == 0)
+    o_ref = o_ref.masked_fill(empty, 0)
+    ob = ob.masked_fill(empty, 0)
+    lse_ref = (m + torch.log2(Ls)).squeeze(-1).masked_fill(empty.squeeze(-1), float("-inf"))
+    lb = (dxm + rho_l / math.log(2) + 2 * ulp_f32(torch.log2(Ls)) + 2 * ulp_f32(m.nan_to_num(0, 0, 0) + torch.log2(Ls)))
+    lb = lb.squeeze(-1).masked_fill(empty.squeeze(-1), 0)
+    return o_ref.permute(0, 2, 1, 3), ob.permute(0, 2, 1, 3), lse_ref, lb
+
+
+def assert_lse_within(lse, ref, bound, name, family=None):
+    fin = torch.isfinite(ref)
+    assert bool(torch.isinf(lse[~fin]).all()), f"{name}: rows without keys need lse = -inf"
+    if bool(fin.any()):
+        return assert_within(lse[fin], ref[fin], bound[fin], name, family=family)
+    return 0.0
+
+
+def onehot_qk(B, H, Sq, Skv, visible, gen, device, mag=64.0):
+    """One-hot q / k (BSHD, bf16; module docstring). Key j of (b, h) gets the code c = perm[b, h, j] (a permutation of the
+    Skv <= 4096 keys, so keys differ between heads and batches) and k_j = mag (e[c % 64] + e[64 + c // 64]): one-hot in the
+    64 slot channels and in the 64 group channels. Each q row is the k row of a random visible target key. Two distinct
+    codes share at most one of the two channels, so the target's logit 2 mag^2 leads every other key's by at least mag^2,
+    whatever the row sees. Returns q, k and the target [B, H, Sq] (-1: no visible key)."""
+    assert Skv <= 64 * 64, "the codes need Skv <= 4096"
+    code = torch.stack([torch.stack([torch.randperm(Skv, generator=gen, device=device) for _ in range(H)]) for _ in range(B)])
+    k = torch.zeros(B, H, Skv, 128, device=device)
+    k.scatter_(-1, (code % 64)[..., None], mag)
+    k.scatter_(-1, (64 + code // 64)[..., None], mag)
+    score = torch.rand(B, H, Sq, Skv, generator=gen, device=device).masked_fill(~visible, -1.0)
+    target = score.argmax(-1).masked_fill(~visible.any(-1), -1)
+    q = k.gather(2, target.clamp_min(0)[..., None].expand(B, H, Sq, 128))
+    q = q.masked_fill((target < 0)[..., None], 0)
+    return q.bfloat16().permute(0, 2, 1, 3), k.bfloat16().permute(0, 2, 1, 3), target

@@ -9,7 +9,8 @@ import pytest
 import torch
 
 import block_bwd_ref as ref
-from test_gpu_linear_bwd import KEY_BIASES, TOL, _ulp_bf16
+from elementwise_ref import ulp_bf16 as _ulp_bf16
+from test_gpu_linear_bwd import KEY_BIASES, TOL
 from util import rel_l2
 
 pytestmark = pytest.mark.gpu

@@ -8,6 +8,7 @@ from ctypes import c_int, c_int64
 import pytest
 import torch
 
+from elementwise_ref import ulp_bf16 as _ulp_bf16
 from util import assert_bf16_parity, rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -61,12 +62,6 @@ def test_strided_x_and_dy():
     _check_grad(dw, dy.float().t() @ x.float(), "dw strided")
     assert torch.equal(db, ops.linear_bwd(x, w, dy.contiguous(), False, False, True)[2])
     assert torch.equal(dx, ops.linear_bwd(x.contiguous(), w, dy.contiguous(), True, False, False)[0])
-
-
-def _ulp_bf16(v):
-    """One bf16 ulp at each value of v (float64): 2^(exponent - 7)."""
-    a = v.abs().clamp_min(2.0 ** -126)
-    return torch.exp2(torch.floor(torch.log2(a)) - 7)
 
 
 @pytest.mark.parametrize("M,N", [(1, 64), (333, 1536), (9450, 5120), (75600, 5120), (1000, 13824)])
