@@ -24,6 +24,7 @@ Implementation differences that do not change results:
 """
 from __future__ import annotations
 
+import functools
 import math
 from dataclasses import dataclass
 
@@ -32,7 +33,7 @@ import torch
 from . import ops
 from .distributed import out_proj_sp
 from .rope import get_rotary_pos_embed
-from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail, refuse_grad
+from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail, refuse_grad, refuse_model_grad
 
 GLOBAL_ATTN_COMPAT_MAX_LATENT_FRAMES = 21  # causal_wanvideo.py:32
 
@@ -248,6 +249,19 @@ def _pad_text(text: torch.Tensor, text_len: int) -> torch.Tensor:
     return text
 
 
+def _inference_only(path: str):
+    """A causal forward (model `self`, or `self.m` for the sequence-parallel one): refused under grad with latents, text or
+    a model tensor requiring grad, run under torch.no_grad() otherwise."""
+    def wrap(fn):
+        @functools.wraps(fn)
+        def run(self, latents, text, *args, **kwargs):
+            refuse_model_grad(path, getattr(self, "m", self), latents, text)
+            with torch.no_grad():
+                return fn(self, latents, text, *args, **kwargs)
+        return run
+    return wrap
+
+
 class CausalWanDiT(WanDiT):
     """CausalWanTransformer3DModel._forward_inference on libfvb200 (batch 1 per call, like the rollout stage)."""
 
@@ -297,11 +311,20 @@ class CausalWanDiT(WanDiT):
             start_frame = 0
         return self.rope_tables(frames, hw, start_frame, device)
 
-    @torch.no_grad()
+    def forward(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor,
+                vsa_sparsity: float | None = None) -> torch.Tensor:
+        """WanDiT's bidirectional forward. Inference only for the causal model: its training (the block-causal mask, the
+        per-frame bf16 modulation backward) is not implemented, so it raises FvbError under grad with an input or a tensor
+        of tensors() requiring grad."""
+        refuse_model_grad("CausalWanDiT", self, latents, text)
+        return super().forward(latents, text, timestep, vsa_sparsity)
+
+    @_inference_only("CausalWanDiT.forward_inference")
     def forward_inference(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor, kv_cache: list,
                           crossattn_cache: list | None, current_start: int = 0, start_frame: int = 0) -> torch.Tensor:
         """latents [1, C, F, H, W] bf16 (the frame block being denoised), text [1, L, text_dim] bf16, timestep [1, F]
-        (one per latent frame). Returns the flow prediction [1, C, F, H, W]."""
+        (one per latent frame). Returns the flow prediction [1, C, F, H, W]. Raises FvbError under grad with an input or a
+        tensor of tensors() requiring grad (there is no causal backward)."""
         cfg = self.cfg
         if not latents.is_cuda:
             raise ops.FvbError("CausalWanDiT.forward_inference needs CUDA tensors (there is no CPU fallback)")
@@ -442,7 +465,7 @@ class SPCausalWanDiT:
         st["hdl"].barrier(channel=1)  # my tokens' heads have arrived from every rank (and everyone is done reading q)
         return block_tail(out_proj_sp(st["back"], blk, x, mod), blk, ctx, mod, cfg, xcache)
 
-    @torch.no_grad()
+    @_inference_only("SPCausalWanDiT.forward_inference")
     def forward_inference(self, latents, text, timestep, kv_cache, crossattn_cache, current_start: int = 0, start_frame: int = 0):
         """Same contract as CausalWanDiT.forward_inference; every rank passes the same inputs and gets the full prediction."""
         import torch.distributed as dist

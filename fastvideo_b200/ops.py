@@ -91,6 +91,26 @@ def linear_bwd(x: torch.Tensor, w: torch.Tensor, dy: torch.Tensor, need_dx: bool
     return dx, dw, db
 
 
+class LinearFn(torch.autograd.Function):
+    """y = bf16(x w^T + b) over rows of x [M, K], w bf16 [N, K], b bf16 [N] or None: forward on fvb_linear_bf16 (the output
+    of the no-grad call, bit for bit), backward on linear_bwd for the inputs that need a gradient (nothing else is
+    launched). An fp32 bias is cast outside, so torch differentiates the cast."""
+
+    @staticmethod
+    def forward(ctx, x, w, b):
+        ctx.save_for_backward(x, w)
+        return linear(x, w, b)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        dy = dy.to(torch.bfloat16)
+        if dy.stride(1) != 1 or dy.stride(0) % 8 != 0:
+            dy = dy.contiguous()
+        need_dx, need_dw, need_db = ctx.needs_input_grad
+        return linear_bwd(x, w, dy, need_dx, need_dw, need_db)
+
+
 def _check_2d(t: torch.Tensor, name: str, shape, dtypes=(torch.bfloat16,)) -> None:
     if not t.is_cuda or t.dtype not in dtypes or t.dim() != 2 or t.stride(1) != 1 or tuple(t.shape) != tuple(shape):
         raise FvbError(f"{name} must be a CUDA {'/'.join(map(str, dtypes))} [{shape[0]}, {shape[1]}] view with unit inner stride")

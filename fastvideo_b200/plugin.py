@@ -362,7 +362,7 @@ def _define():
 
 def linear_forward(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None) -> torch.Tensor:
     """Fvb200LinearMethod.apply (UnquantizedLinearMethod's F.linear, layers/linear.py:146-156): bf16(x w^T + bias) over the
-    last axis of x on fvb_linear_bf16. With grad enabled and x, w or bias requiring grad it runs _LinearFn (the same
+    last axis of x on fvb_linear_bf16. With grad enabled and x, w or bias requiring grad it runs ops.LinearFn (the same
     forward call, backward on fvb_linear_dgrad_bf16 / fvb_linear_wgrad_bf16 / fvb_bias_grad_bf16); otherwise the plain call."""
     if not x.is_cuda:
         raise FvbError("fvb200_bf16 linear needs CUDA tensors (there is no CPU fallback)")
@@ -373,30 +373,10 @@ def linear_forward(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None =
         x2 = x2.contiguous()
     b = None if bias is None else bias.to(torch.bfloat16)
     if torch.is_grad_enabled() and (x.requires_grad or w.requires_grad or (b is not None and b.requires_grad)):
-        out = _LinearFn.apply(x2, w, b)
+        out = ops.LinearFn.apply(x2, w, b)
     else:
         out = ops.linear(x2, w, b)
     return out.reshape(*x.shape[:-1], w.shape[0])
-
-
-class _LinearFn(torch.autograd.Function):
-    """y = bf16(x w^T + b) over rows of x [M, K], w bf16 [N, K], b bf16 [N] or None: forward on fvb_linear_bf16 (the output
-    of the no-grad call, bit for bit), backward on ops.linear_bwd for the inputs that need a gradient (nothing else is
-    launched). An fp32 bias is cast outside, so torch differentiates the cast."""
-
-    @staticmethod
-    def forward(ctx, x, w, b):
-        ctx.save_for_backward(x, w)
-        return ops.linear(x, w, b)
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, w = ctx.saved_tensors
-        dy = dy.to(torch.bfloat16)
-        if dy.stride(1) != 1 or dy.stride(0) % 8 != 0:
-            dy = dy.contiguous()
-        need_dx, need_dw, need_db = ctx.needs_input_grad
-        return ops.linear_bwd(x, w, dy, need_dx, need_dw, need_db)
 
 
 def rms_norm_forward_cuda(self, x: torch.Tensor, residual: torch.Tensor | None = None):

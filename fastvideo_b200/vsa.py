@@ -88,6 +88,10 @@ class _VideoSparseAttnFn(torch.autograd.Function):
     block_map (bool [B, H, nblk, nblk], or None for the top-k of the block scores) fixes the selection; it is how the
     tests reach q blocks without keys, which top-k never produces."""
 
+    # the order of ctx.saved_tensors (callers that run forward / backward with a stand-in ctx read them by these names)
+    SAVED = ("q", "k", "v", "gate", "vbs", "q_ct", "k_ct", "v_c", "attn", "out_c", "out_s", "lse", "q2k_idx", "q2k_num",
+             "block_map", "block_off", "row_block")
+
     @staticmethod
     def forward(ctx, q, k, v, gate, vbs, topk, block_map, block_off=None, row_block=None):
         if SPARSE_KERNEL != "ws":

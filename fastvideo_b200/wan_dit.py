@@ -180,20 +180,24 @@ class WanBlock:
         return {n: getattr(self, n) for n in names}
 
     @staticmethod
-    def to_reference_names(t: dict, prefix: str = "") -> dict:
+    def to_reference_names(t: dict, prefix: str = "", like: dict | None = None) -> dict:
         """{fused name: tensor} (WanBlock.tensors(), or the same keys holding gradients) -> {reference name: tensor}: the
-        fused QKV(+gate) / text KV / image KV rows are split back into their projections (views, no copies)."""
+        fused QKV(+gate) / text KV / image KV rows are split back into their projections (views, no copies). An entry may be
+        None (the .grad of a tensor that is not trained): its reference names map to None, and `like` (the block's own
+        tensors()) gives the shapes the split needs."""
         out = {}
-        D = t["w_o"].shape[0]
-        qkv = ["to_q", "to_k", "to_v", "to_gate_compress"][:t["w_qkv"].shape[0] // D]
+        s = t if like is None else like
+        D = s["w_o"].shape[0]
+        rows = lambda src, a, b: None if t[src] is None else t[src][a:b]
+        qkv = ["to_q", "to_k", "to_v", "to_gate_compress"][:s["w_qkv"].shape[0] // D]
         for i, n in enumerate(qkv):
-            out[n + ".weight"] = t["w_qkv"][i * D:(i + 1) * D]
-            out[n + ".bias"] = t["b_qkv"][i * D:(i + 1) * D]
+            out[n + ".weight"] = rows("w_qkv", i * D, (i + 1) * D)
+            out[n + ".bias"] = rows("b_qkv", i * D, (i + 1) * D)
         for src, dst in (("w_kv2", "attn2.to_{}.weight"), ("b_kv2", "attn2.to_{}.bias")):
-            out[dst.format("k")], out[dst.format("v")] = t[src][:D], t[src][D:]
+            out[dst.format("k")], out[dst.format("v")] = rows(src, 0, D), rows(src, D, None)
         if "w_kv_img" in t:
             for src, dst in (("w_kv_img", "attn2.add_{}_proj.weight"), ("b_kv_img", "attn2.add_{}_proj.bias")):
-                out[dst.format("k")], out[dst.format("v")] = t[src][:D], t[src][D:]
+                out[dst.format("k")], out[dst.format("v")] = rows(src, 0, D), rows(src, D, None)
             out["attn2.norm_added_k.weight"] = t["norm_k_img"]
         plain = {"norm_q": "norm_q.weight", "norm_k": "norm_k.weight", "w_o": "to_out.weight", "b_o": "to_out.bias",
                  "norm2_w": "self_attn_residual_norm.norm.weight", "norm2_b": "self_attn_residual_norm.norm.bias",
@@ -365,18 +369,24 @@ def block_tail(y: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulatio
 
 
 def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torch.Tensor, lay: TokenLayout,
-                  cfg: WanDiTConfig) -> torch.Tensor:
+                  cfg: WanDiTConfig, checkpoint: bool = False) -> torch.Tensor:
     """x: [S, D] bf16 (one sample), ctx: [L, D] bf16 text states, temb6: [1, 6, D] (timestep_proj). Returns [S, D].
     Differentiable (in x, ctx, temb6 and every tensor of blk.tensors()) when grad is enabled and one of them requires grad:
-    the block then runs _WanBlockFn, whose forward is this same body (block_body) and returns the same bits."""
+    the block then runs _WanBlockFn, whose forward is this same body (block_body) and returns the same bits.
+    checkpoint: under grad, keep only the block input, the modulation and the self-attention results
+    (checkpoint_bytes_per_block); the backward re-runs the block around the saved self-attention first."""
     if torch.is_grad_enabled() and _any_requires_grad(blk, x, ctx, temb6):
-        return _block_forward_grad(x, blk, ctx, temb6, lay, cfg)
+        return _block_forward_grad(x, blk, ctx, temb6, lay, cfg, checkpoint)
     return block_body(x, blk, ctx, Modulation.fp32(blk, temb6), lay, cfg)
 
 
 def block_body(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulation, lay: TokenLayout, cfg: WanDiTConfig,
-               keep: dict | None = None) -> torch.Tensor:
-    """The single-rank block: self-attention (wanvideo.py:393-415), then block_tail. `keep`: see _keep."""
+               keep: dict | None = None, attn: dict | None = None, replay: bool = False) -> torch.Tensor:
+    """The single-rank block: self-attention (wanvideo.py:393-415), then block_tail. `keep`: see _keep. `attn` (the
+    checkpointed block, _WanBlockFn) records the self-attention results: dense "a" and "lse"; VSA the tensors
+    _VideoSparseAttnFn saves besides q / k / v / gate, under their _VideoSparseAttnFn.SAVED names. With `replay` those
+    results are used instead of launching the self-attention (for VSA the output is recombined from the saved branches
+    and the recomputed gate by the same fvb_vsa_combine call, so the same bits)."""
     S, D = x.shape
     H, d = cfg.num_attention_heads, cfg.head_dim
     n1 = mod.norm1(x, cfg.eps)
@@ -389,15 +399,26 @@ def block_body(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulatio
     v = qkv[:, 2 * D:3 * D].unflatten(1, (H, d)).unsqueeze(0)
     if cfg.vsa:
         gate = qkv[:, 3 * D:4 * D].unflatten(1, (H, d)).unsqueeze(0)
-        if keep is None:
+        if replay:
+            a = ops.vsa_combine(attn["out_s"], attn["out_c"], gate, row_block=lay.row_block)
+            _keep(keep, vsa=(q, k, v, gate, *(attn[n] for n in vsa._VideoSparseAttnFn.SAVED[4:])))
+        elif keep is None and attn is None:
             a = vsa.video_sparse_attn_bshd(q, k, v, lay.vbs, lay.topk, gate=gate, block_off=lay.block_off,
                                            row_block=lay.row_block, attn_8bit=cfg.attention_8bit)
         else:  # the same kernels in the same order (bit-identical), keeping what the VSA backward needs
             vctx = _SavedCtx()
             a = vsa._VideoSparseAttnFn.forward(vctx, q, k, v, gate, lay.vbs, lay.topk, None, lay.block_off, lay.row_block)
-            keep["vsa"] = vctx.saved_tensors
+            _keep(keep, vsa=vctx.saved_tensors)
+            if attn is not None:
+                attn.update(zip(vsa._VideoSparseAttnFn.SAVED[4:], vctx.saved_tensors[4:]))
     elif cfg.attention_8bit:
         a = ops.attention_8bit(ops.quantize_attention_8bit(q, k, v), d ** -0.5)
+    elif replay:
+        a = attn["a"]
+        _keep(keep, lse=attn["lse"])
+    elif attn is not None:
+        a, attn["lse"] = ops.attention(q, k, v, softmax_scale=d ** -0.5, return_lse=True)
+        attn["a"] = a = a.reshape(S, D)
     else:
         a = _attention_kept(keep, "lse", q, k, v, d ** -0.5)
     _keep(keep, a=a.reshape(S, D))
@@ -423,10 +444,11 @@ def refuse_grad(path: str, blk: WanBlock, *inputs) -> None:
 
 _BLOCK_TENSORS = ("w_qkv", "b_qkv", "norm_q", "norm_k", "w_o", "b_o", "norm2_w", "norm2_b", "w_q2", "b_q2", "w_kv2", "b_kv2",
                   "norm_q2", "norm_k2", "w_o2", "b_o2", "w_1", "b_1", "w_2", "b_2", "w_kv_img", "b_kv_img", "norm_k_img")
-_FN_LEAD = 11  # _WanBlockFn inputs before the block tensors: x, ctx, six modulation vectors, blk, lay, cfg
+_FN_LEAD = 12  # _WanBlockFn inputs before the block tensors: x, ctx, six modulation vectors, blk, lay, cfg, checkpoint
 
 
-def _block_forward_grad(x, blk: WanBlock, ctx, temb6, lay: TokenLayout, cfg: WanDiTConfig) -> torch.Tensor:
+def _require_trainable(blk: WanBlock, cfg: WanDiTConfig) -> None:
+    """Raise FvbError for a block configuration the backward does not cover."""
     if not blk.trainable or cfg.attention_8bit:
         raise ops.FvbError("the Wan block backward covers bf16 linears and bf16 attention: fp8_linears, int8_weights / "
                            "int8_activations and attention_8bit run without grad only")
@@ -436,9 +458,28 @@ def _block_forward_grad(x, blk: WanBlock, ctx, temb6, lay: TokenLayout, cfg: Wan
             raise ops.FvbError(f"the Wan block backward needs bf16 RMSNorm weights ({n} is {t.dtype})")
     if cfg.vsa and vsa.SPARSE_KERNEL != "ws":
         raise ops.FvbError("the VSA backward needs the block-list sparse kernel (FVB_VSA_KERNEL=ws)")
+
+
+def _block_forward_grad(x, blk: WanBlock, ctx, temb6, lay: TokenLayout, cfg: WanDiTConfig, checkpoint: bool) -> torch.Tensor:
+    _require_trainable(blk, cfg)
     mod = Modulation.fp32(blk, temb6)  # torch ops: autograd carries the six vectors back to scale_shift_table and temb6
     return _WanBlockFn.apply(x, ctx, mod.shift_msa, mod.scale_msa, mod.gate_msa, mod.c_shift, mod.c_scale, mod.c_gate, blk, lay,
-                             cfg, *(getattr(blk, n) for n in _BLOCK_TENSORS))
+                             cfg, checkpoint, *(getattr(blk, n) for n in _BLOCK_TENSORS))
+
+
+def checkpoint_bytes_per_block(S: int, D: int, H: int, n_tiles: int = 0) -> int:
+    """Bytes a checkpointed block (block_forward(..., checkpoint=True)) keeps from its forward to its backward, for S
+    tokens of width D in H heads: the bf16 input, the fp32 modulation vectors, and the self-attention results. Dense (n_tiles
+    0): the bf16 output and the fp32 LSE. VSA (n_tiles tiles): the sparse branch's bf16 output and fp32 LSE, the block
+    means (q, k transposed with rows padded to 8 tiles; v) and the compression output, the block-score softmax (rows
+    padded to 8), the int32 index lists and counts and the bool block map. The layout tables and the text states are
+    shared by every block and not counted."""
+    n, n8 = n_tiles, (n_tiles + 7) // 8 * 8
+    common = 2 * S * D + 6 * 4 * D + 2 * S * D + 4 * S * H
+    if not n_tiles:
+        return common
+    d = D // H
+    return common + H * (2 * 2 * d * n8 + 2 * 2 * n * d + 2 * n * n8 + 4 * n * n + 4 * n + n * n)
 
 
 class _SavedCtx:
@@ -453,15 +494,23 @@ class _WanBlockFn(torch.autograd.Function):
     """block_forward with autograd. The forward is block_body with a `keep` dict: the same kernel calls (same bits), plus
     storage for the backward -- the pre-norm q / k / q2 / k2 (cloned before the in-place norms), the attention LSEs, and the
     pre-epilogue bf16 y of the fc_in / to_out / fc_out GEMMs (fvb_linear_bf16_aux). The backward is torch autograd's for the
-    reference block (DESIGN.md "Wan block backward"); weight / bias / context gradients that no input needs are skipped."""
+    reference block (DESIGN.md "Wan block backward"); weight / bias / context gradients that no input needs are skipped.
+    With `checkpoint` the forward keeps only x, ctx, the modulation vectors and the self-attention results (block_body's
+    `attn`); the backward first re-runs block_body with a `keep` dict around those results (no self-attention launch) and
+    then proceeds as without checkpoint. The forward kernels are deterministic, so the re-run keeps the same bits and the
+    gradients are those of the forward without checkpoint."""
 
     @staticmethod
-    def forward(fctx, x, ctx, shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, blk, lay, cfg, *params):
-        keep = {}
+    def forward(fctx, x, ctx, shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, blk, lay, cfg, checkpoint, *params):
+        keep, attn = (None, {}) if checkpoint else ({}, None)
         mod = Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate)
-        out = block_body(x.detach(), blk, ctx.detach(), mod, lay, cfg, keep)
+        out = block_body(x.detach(), blk, ctx.detach(), mod, lay, cfg, keep, attn)
+        fctx.blk, fctx.lay, fctx.cfg, fctx.checkpoint = blk, lay, cfg, checkpoint
+        if checkpoint:
+            fctx.names = tuple(attn)
+            fctx.save_for_backward(x, ctx, scale_msa, gate_msa, c_scale, c_gate, shift_msa, c_shift, *attn.values())
+            return out
         vsa_saved = keep.pop("vsa", ())
-        fctx.blk, fctx.lay, fctx.cfg = blk, lay, cfg
         fctx.names = tuple(keep)
         fctx.save_for_backward(x, ctx, scale_msa, gate_msa, c_scale, c_gate, *keep.values(), *vsa_saved)
         return out
@@ -469,10 +518,17 @@ class _WanBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(fctx, dout):
         x, ctx, scale_msa, gate_msa, c_scale, c_gate = fctx.saved_tensors[:6]
-        names = fctx.names
-        kp = dict(zip(names, fctx.saved_tensors[6:6 + len(names)]))
-        vsa_saved = fctx.saved_tensors[6 + len(names):]
         blk, lay, cfg = fctx.blk, fctx.lay, fctx.cfg
+        if fctx.checkpoint:
+            shift_msa, c_shift, *saved = fctx.saved_tensors[6:]
+            kp = {}
+            block_body(x, blk, ctx, Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate), lay, cfg, kp,
+                       dict(zip(fctx.names, saved)), replay=True)
+            vsa_saved = kp.pop("vsa", ())
+        else:
+            names = fctx.names
+            kp = dict(zip(names, fctx.saved_tensors[6:6 + len(names)]))
+            vsa_saved = fctx.saved_tensors[6 + len(names):]
         need = lambda n: fctx.needs_input_grad[_FN_LEAD + _BLOCK_TENSORS.index(n)]
         S, D = x.shape
         H, d = cfg.num_attention_heads, cfg.head_dim
@@ -547,12 +603,94 @@ class _WanBlockFn(torch.autograd.Function):
                                                         want_dw=need("norm_q") or need("norm_k"))
         dn1, g["w_qkv"], g["b_qkv"] = ops.linear_bwd(kp["n1"], blk.w_qkv, dqkv, need_dw=need("w_qkv"), need_db=need("b_qkv"))
         dx, d_scale_msa, d_shift_msa = ops.layernorm_modulate_bwd(x, dn1, scale=scale_msa, gin=dy, eps=eps)
-        return (dx, dctx, d_shift_msa, d_scale_msa, d_gate_msa, d_cshift, d_cscale, d_cgate, None, None, None,
+        return (dx, dctx, d_shift_msa, d_scale_msa, d_gate_msa, d_cshift, d_cscale, d_cgate, None, None, None, None,
                 *(g.get(n) if need(n) else None for n in _BLOCK_TENSORS))
 
 
+def _requires_grad(*tensors) -> bool:
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+def _any_model_tensor_requires_grad(model, *inputs) -> bool:
+    """Grad enabled and an input or a tensor of model.tensors() requires grad (quantised weights are not tensors)."""
+    return torch.is_grad_enabled() and _requires_grad(*inputs, *(t for t in model.tensors().values()
+                                                                 if isinstance(t, torch.Tensor)))
+
+
+def refuse_model_grad(path: str, model, *inputs) -> None:
+    """Raise FvbError when a model forward without a backward would run with grad enabled and an input or a tensor of
+    model.tensors() requiring grad."""
+    if _any_model_tensor_requires_grad(model, *inputs):
+        raise ops.FvbError(f"{path} has no backward: run it under torch.no_grad(), or train the single-rank model "
+                           "(WanDiT.forward)")
+
+
+def _linear(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """ops.linear over the last axis of x; through ops.LinearFn when grad is enabled and x, w or b requires grad."""
+    if not _requires_grad(x, w, b):
+        return ops.linear(x, w, b)
+    return ops.LinearFn.apply(x.reshape(-1, x.shape[-1]), w, b).view(*x.shape[:-1], w.shape[0])
+
+
+class _GeluMlpFn(torch.autograd.Function):
+    """y = fc_out(gelu_tanh(fc_in(x))) over rows of x [M, K] (the text embedder, wanvideo.py:100-135 / mlp.py:47-51): fc_in
+    with its GELU epilogue on fvb_linear_bf16_aux (which also keeps the pre-GELU h), fc_out on fvb_linear_bf16, the no-grad
+    calls' bits. The backward is the block feed-forward's: fc_out's weight / bias gradients on linear_bwd, dh = bf16(bf16(dy
+    w_out) gelu'(h)) in one GEMM epilogue (fvb_linear_dgrad_gelu_bf16, which needs fc_out's weight, hence one Function for
+    both linears), then linear_bwd of fc_in."""
+
+    @staticmethod
+    def forward(ctx, x, w_in, b_in, w_out, b_out):
+        f, h = ops.linear_aux(x, w_in, b_in, ops.EPI_BIAS_GELU_TANH)
+        ctx.save_for_backward(x, w_in, w_out, f, h)
+        return ops.linear(f, w_out, b_out)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w_in, w_out, f, h = ctx.saved_tensors
+        need_x, need_w_in, need_b_in, need_w_out, need_b_out = ctx.needs_input_grad
+        dy = dy.to(torch.bfloat16).contiguous()
+        _, dw_out, db_out = ops.linear_bwd(f, w_out, dy, need_dx=False, need_dw=need_w_out, need_db=need_b_out)
+        dx = dw_in = db_in = None
+        if need_x or need_w_in or need_b_in:
+            dh = ops.linear_dgrad_gelu(dy, w_out, h)
+            dx, dw_in, db_in = ops.linear_bwd(x, w_in, dh, need_dx=need_x, need_dw=need_w_in, need_db=need_b_in)
+        return dx, dw_in, db_in, dw_out, db_out
+
+
+class _HeadNormFn(torch.autograd.Function):
+    """norm_out: n = bf16(bf16(LN(x)) (1 + scale) + shift) (ops.layernorm_modulate with round_ln, the no-grad call's bits);
+    backward on fvb_layernorm_modulate_bwd (dx bf16, d_scale / d_shift fp32)."""
+
+    @staticmethod
+    def forward(ctx, x, scale, shift, eps):
+        ctx.save_for_backward(x, scale)
+        ctx.eps = eps
+        return ops.layernorm_modulate(x, scale, shift, round_ln=True, eps=eps)
+
+    @staticmethod
+    def backward(ctx, dn):
+        x, scale = ctx.saved_tensors
+        dx, d_scale, d_shift = ops.layernorm_modulate_bwd(x, dn.to(torch.bfloat16).contiguous(), scale=scale, round_ln=True,
+                                                          eps=ctx.eps)
+        return dx, d_scale, d_shift, None
+
+
+# WanDiT's own trainable tensors (attribute name -> reference parameter name); the blocks' follow under blocks.{i}.
+_MODEL_TENSORS = {
+    "w_patch": "patch_embedding.proj.weight", "b_patch": "patch_embedding.proj.bias",
+    "w_t1": "condition_embedder.time_embedder.mlp.fc_in.weight", "b_t1": "condition_embedder.time_embedder.mlp.fc_in.bias",
+    "w_t2": "condition_embedder.time_embedder.mlp.fc_out.weight", "b_t2": "condition_embedder.time_embedder.mlp.fc_out.bias",
+    "w_tm": "condition_embedder.time_modulation.linear.weight", "b_tm": "condition_embedder.time_modulation.linear.bias",
+    "w_x1": "condition_embedder.text_embedder.fc_in.weight", "b_x1": "condition_embedder.text_embedder.fc_in.bias",
+    "w_x2": "condition_embedder.text_embedder.fc_out.weight", "b_x2": "condition_embedder.text_embedder.fc_out.bias",
+    "scale_shift_table": "scale_shift_table", "w_out": "proj_out.weight", "b_out": "proj_out.bias"}
+
+
 class WanDiT:
-    """WanTransformer3DModel on libfvb200 (inference forward only)."""
+    """WanTransformer3DModel on libfvb200: the denoising forward, and its backward when grad is enabled and latents, text or
+    a tensor of tensors() requires grad (forward(..., checkpoint=True) for block activation checkpointing). The
+    sequence-parallel (distributed.SPWanDiT) and causal (causal_wan.CausalWanDiT) models reuse its pieces for inference."""
 
     def __init__(self, cfg: WanDiTConfig, state_dict: dict, blocks: list | None = None):
         self.cfg = cfg
@@ -590,6 +728,33 @@ class WanDiT:
             del sd
         return cls(cfg, random_state_dict(cfg, device, seed, layers=0), blocks=blocks)
 
+    def tensors(self) -> dict:
+        """Every trainable tensor, by attribute name: the model's own (patch embedding, condition embedder, head) and each
+        block's WanBlock.tensors() under "blocks.{i}.". Each is a leaf an optimizer can step; set requires_grad on the ones
+        to train. to_reference_names maps this dict, or the same keys holding gradients, to the reference names."""
+        out = {n: getattr(self, n) for n in _MODEL_TENSORS}
+        for i, blk in enumerate(self.blocks):
+            out.update({f"blocks.{i}.{n}": t for n, t in blk.tensors().items()})
+        return out
+
+    def to_reference_names(self, t: dict) -> dict:
+        """{name: tensor} as tensors() returns it, or the same keys holding gradients -> {reference parameter name: tensor},
+        every one a view of the given tensor in the reference's shape (w_patch [D, C * pt * ph * pw] becomes
+        patch_embedding.proj.weight [D, C, pt, ph, pw]). None entries (the .grad of a tensor that is not trained) map to
+        None. WanDiT(cfg, model.to_reference_names(model.tensors())) rebuilds the model."""
+        out = {ref: t[n] for n, ref in _MODEL_TENSORS.items()}
+        w = t["w_patch"]
+        if w is not None:
+            out["patch_embedding.proj.weight"] = w.view(w.shape[0], self.cfg.in_channels, *self.cfg.patch_size)
+        blocks: dict = {}
+        for k, v in t.items():
+            if k.startswith("blocks."):
+                i, n = k[len("blocks."):].split(".", 1)
+                blocks.setdefault(int(i), {})[n] = v
+        for i in sorted(blocks):
+            out.update(WanBlock.to_reference_names(blocks[i], f"blocks.{i}.", like=self.blocks[i].tensors()))
+        return out
+
     # ---- pieces of WanTransformer3DModel.forward ----
     def layout(self, seq_shape, device, vsa_sparsity=None) -> TokenLayout:
         key = (tuple(seq_shape), vsa_sparsity if self.cfg.vsa else None)
@@ -608,10 +773,14 @@ class WanDiT:
         freqs = self._t_freqs
         args = timestep[:, None].float() * freqs[None]
         t_freq = torch.cat([torch.cos(args), torch.sin(args)], dim=-1).to(torch.bfloat16)
-        h = ops.linear(t_freq, self.w_t1, self.b_t1)
-        temb = ops.linear(torch.nn.functional.silu(h), self.w_t2, self.b_t2)          # [B, D]
-        tproj = ops.linear(torch.nn.functional.silu(temb), self.w_tm, self.b_tm)       # [B, 6D]
-        ctx = ops.linear(ops.linear(text, self.w_x1, self.b_x1, ops.EPI_BIAS_GELU_TANH), self.w_x2, self.b_x2)
+        h = _linear(t_freq, self.w_t1, self.b_t1)
+        temb = _linear(torch.nn.functional.silu(h), self.w_t2, self.b_t2)          # [B, D]
+        tproj = _linear(torch.nn.functional.silu(temb), self.w_tm, self.b_tm)       # [B, 6D]
+        if _requires_grad(text, self.w_x1, self.b_x1, self.w_x2, self.b_x2):
+            ctx = _GeluMlpFn.apply(text.reshape(-1, text.shape[-1]), self.w_x1, self.b_x1, self.w_x2,
+                                   self.b_x2).view(*text.shape[:-1], -1)
+        else:
+            ctx = ops.linear(ops.linear(text, self.w_x1, self.b_x1, ops.EPI_BIAS_GELU_TANH), self.w_x2, self.b_x2)
         return temb, tproj.unflatten(1, (6, -1)), ctx
 
     def patches(self, latents: torch.Tensor) -> torch.Tensor:
@@ -627,7 +796,7 @@ class WanDiT:
         x = self.patches(latents)
         if lay.perm is not None:
             x = x[:, lay.perm]
-        return ops.linear(x.contiguous(), self.w_patch, self.b_patch)
+        return _linear(x.contiguous(), self.w_patch, self.b_patch)
 
     def head(self, x: torch.Tensor, temb: torch.Tensor, lay: TokenLayout, batch_index: int = 0) -> torch.Tensor:
         """norm_out + proj_out for one sample (wanvideo.py:746-759). x: [S, D] -> [S, C*pt*ph*pw]."""
@@ -637,8 +806,11 @@ class WanDiT:
         # (1.0 + scale) is evaluated in e's dtype (bf16) before it meets the fp32 LN output (layernorm.py:262-268):
         # scale' = bf16(1 + scale) - 1 is exact in fp32 and makes the kernel's fp32 (1 + scale') equal to it
         scale = ((1.0 + e[:, 1]).float() - 1.0).reshape(D).contiguous()
-        n = ops.layernorm_modulate(x, scale, shift, round_ln=True, eps=self.cfg.eps)
-        return ops.linear(n, self.w_out, self.b_out)
+        if _requires_grad(x, scale, shift):
+            n = _HeadNormFn.apply(x, scale, shift, self.cfg.eps)
+        else:
+            n = ops.layernorm_modulate(x, scale, shift, round_ln=True, eps=self.cfg.eps)
+        return _linear(n, self.w_out, self.b_out)
 
     def unpatchify(self, y: torch.Tensor, lay: TokenLayout) -> torch.Tensor:
         """[B, S, C*pt*ph*pw] (layout order) -> [B, C, T, H, W] (wanvideo.py:761-764)."""
@@ -650,13 +822,18 @@ class WanDiT:
         y = y.reshape(B, T, Hh, Ww, pt, ph, pw, -1).permute(0, 7, 1, 4, 2, 5, 3, 6)
         return y.flatten(6, 7).flatten(4, 5).flatten(2, 3)
 
-    @torch.no_grad()
     def forward(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor,
-                vsa_sparsity: float | None = None) -> torch.Tensor:
-        """latents [B, C, T, H, W] bf16, text [B, L, text_dim] bf16, timestep [B] -> noise prediction, same shape."""
+                vsa_sparsity: float | None = None, checkpoint: bool = False) -> torch.Tensor:
+        """latents [B, C, T, H, W] bf16, text [B, L, text_dim] bf16, timestep [B] -> noise prediction, same shape.
+        Differentiable in latents, text and every tensor of tensors() when grad is enabled and one of them requires grad
+        (the output is the same bits as without grad); otherwise the plain inference calls. checkpoint: under grad, each
+        block keeps only its input, its modulation and its self-attention results (block_forward)."""
         cfg = self.cfg
         if not latents.is_cuda:
             raise ops.FvbError("WanDiT.forward needs CUDA tensors (there is no CPU fallback)")
+        if _any_model_tensor_requires_grad(self, latents, text):
+            for blk in self.blocks:  # refused before anything runs, even when only the model's own tensors require grad
+                _require_trainable(blk, cfg)
         B = latents.shape[0]
         pt, ph, pw = cfg.patch_size
         seq_shape = (latents.shape[2] // pt, latents.shape[3] // ph, latents.shape[4] // pw)
@@ -667,6 +844,6 @@ class WanDiT:
         for b in range(B):
             xb = x[b]
             for blk in self.blocks:
-                xb = block_forward(xb, blk, ctx[b], tproj[b:b + 1], lay, cfg)
+                xb = block_forward(xb, blk, ctx[b], tproj[b:b + 1], lay, cfg, checkpoint)
             outs.append(self.head(xb, temb, lay, b))
         return self.unpatchify(torch.stack(outs, 0), lay)
