@@ -39,6 +39,30 @@ Attention constructions (tie_attention_ref), exact for the bf16 kernel's online 
     Random inputs use attention_bound: the fp32 logit error (c * sum |q k| from the QK^T chain, plus 3 roundings of
     x) is amplified through exp2 into a relative error rho of each p; P's bf16 rounding (relative 2^-8) and the P V chain
     add relative errors on each p |v|; the output rounds once more (half a bf16 ulp).
+
+Attention backward (include/fvb200.h: delta_i = sum dO o, P = ex2(fma(s, scale_log2, -lse)), dS = P (dP - delta) scale,
+dV = sum bf16(P) dO, dK = sum bf16(dS) q, dQ = sum bf16(dS) k). o and lse are inputs of the backward, so a test chooses
+them; they need not come from the forward. bwd_exact_ref covers three constructions (bwd_inputs), all at softmax_scale
+2^-4, with dO on the grid and v, o on the grid with two non-zero channels per row (|a| <= 3). Then dP - delta = dO (v - o)
+is at most 4 * 15 * 3 = 180 quanta of 2^-8, so dP, delta and their difference are exact in fp32, dS = (dP - delta) 2^-4
+has at most 8 significant bits (bf16(dS) == dS), and every sum of the second GEMMs is an integer number of quanta below
+2^24, exact in any order:
+    one-hot:   q, k from onehot_qk, lse = fl(8192 scale_log2) for rows that see a key (-inf for the others). 8192 is a
+               power of two, so fma(8192, scale_log2, -lse) is exactly 0 and ex2(0) = 1; every other visible key sits at
+               least 4096 scale_log2 (369 at 2^-4) lower and gets P = 0. dV_j = sum over the rows that target j of dO_i,
+               dQ_i = bf16(dS_it) k_t, dK_j = sum over the rows that target j of bf16(dS_ij) q_i: a wrong row, head, batch,
+               tile or list entry gives other bits.
+    uniform-q: q = 0, lse = 0: every visible pair has P = 1, so dV_j sums dO over every row that sees j and dQ_i sums
+               bf16(dS_ij) k_j over every key row i sees; one masked key counted or one visible key dropped changes both.
+    uniform-k: k = 0, lse = 0: the same for dK.
+    bwd_exact_ref asserts these premises (integer logits, x either 0 or at least 150 below, bf16(dS) == dS, every partial
+    sum below 2^24 quanta) and replays the fp32 roundings of dS with torch fp32 ops.
+Random inputs use attention_bwd_bound, on the kernel's own inputs (the fp32 lse passed, scale_log2 = fl(fl(scale)
+fl(log2 e))): the QK^T and dO V^T chains (acc_coeff(128) sum |q k|, likewise for dP), fma's rounding and exp2's relative
+error 2^-22 (ex2.approx.f32 in the wgmma kernels; exp2f, at most 2 fp32 ulp, in the mma.sync kernels: 2^-22 covers both),
+delta's fp32 sum (128 U32 sum |dO o|), the roundings of P (dP - delta) scale, the bf16 rounding of P and dS (half an ulp
+each), the second GEMM's chain (acc_coeff(rows walked) sum |bf16(.)| |operand|) and the final bf16 store, element by
+element as [B, H, Sq, Skv] fp64 tensors followed by a matmul with |operand|.
 """
 import math
 
@@ -422,3 +446,186 @@ def onehot_qk(B, H, Sq, Skv, visible, gen, device, mag=64.0):
     q = k.gather(2, target.clamp_min(0)[..., None].expand(B, H, Sq, 128))
     q = q.masked_fill((target < 0)[..., None], 0)
     return q.bfloat16().permute(0, 2, 1, 3), k.bfloat16().permute(0, 2, 1, 3), target
+
+
+def make_qkv(B, Sq, Skv, H, layout, device):
+    """Uninitialised q [B, Sq, H, 128] and k, v [B, Skv, H, 128] views in one of three layouts."""
+    if layout == "bshd":
+        return (torch.empty(B, Sq, H, 128, dtype=torch.bfloat16, device=device),
+                *(torch.empty(B, Skv, H, 128, dtype=torch.bfloat16, device=device) for _ in range(2)))
+    if layout == "bhsd":
+        return (torch.empty(B, H, Sq, 128, dtype=torch.bfloat16, device=device).transpose(1, 2),
+                *(torch.empty(B, H, Skv, 128, dtype=torch.bfloat16, device=device).transpose(1, 2) for _ in range(2)))
+    qb = torch.empty(B, Sq, 3, H, 128, dtype=torch.bfloat16, device=device)  # fused [B, S, 3, H, 128] GEMM outputs
+    kvb = torch.empty(B, Skv, 3, H, 128, dtype=torch.bfloat16, device=device)
+    return qb[:, :, 0], kvb[:, :, 1], kvb[:, :, 2]
+
+
+def block_lists(sel):
+    """bool [b, h, nqb, nkb] -> ascending lists int32 [b, h, nqb, nkb] (-1 padded) and counts [b, h, nqb]."""
+    num = sel.sum(-1).to(torch.int32)
+    key = torch.where(sel, torch.arange(sel.shape[-1], device=sel.device), sel.shape[-1])
+    idx = key.sort(-1).values.to(torch.int32)
+    idx[idx == sel.shape[-1]] = -1
+    return idx.contiguous(), num.contiguous()
+
+
+def select_blocks(nqb, nkb, topk, bcast, g, device):
+    """bool [b, h, nqb, nkb] with topk blocks per q block; q block 3 selects only the empty kv blocks 1 and 6."""
+    b, h = {"none": (2, 3), "batch": (1, 3), "both": (1, 1)}[bcast]
+    sel = torch.zeros(b, h, nqb, nkb, dtype=torch.bool, device=device)
+    score = torch.rand(b, h, nqb, nkb, generator=g, device=device)
+    sel.scatter_(-1, score.topk(topk, -1).indices, True)
+    sel[:, :, 3] = False
+    sel[:, :, 3, [1, 6]] = True
+    return sel
+
+
+# ------------------------------------------------------------------------------------------------ attention backward
+def _bhsd64(*ts):
+    return (t.permute(0, 2, 1, 3).double() for t in ts)
+
+
+def _few_channels(shape, gen, device, n=2, lim=3):
+    """bf16 grid rows a * 2^-4 (|a| <= lim) with n non-zero channels each, at random places."""
+    a = grid_bf16(shape, gen, device, lim=lim)
+    keep = torch.rand(tuple(shape), generator=gen, device=device).topk(n, -1).indices
+    return torch.zeros_like(a).scatter_(-1, keep, a.gather(-1, keep))
+
+
+def lse_and_out(q, k, v, visible, softmax_scale):
+    """The forward's LSE (fp64, rounded to fp32; -inf for rows without keys) and o (bf16) of q, k, v (BSHD) under visible,
+    at the kernel's fp32 scale_log2."""
+    qh, kh, vh = _bhsd64(q, k, v)
+    x = ((qh @ kh.transpose(-1, -2)) * scale_log2_f32(softmax_scale)).masked_fill(~visible, float("-inf"))
+    m = x.amax(-1, keepdim=True)
+    m = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
+    p = torch.exp2(x - m)
+    L = p.sum(-1, keepdim=True)
+    lse = (m + torch.log2(L)).squeeze(-1).float()
+    o = ((p @ vh) / L.clamp_min(1e-300)).permute(0, 2, 1, 3).bfloat16()
+    return lse, o
+
+
+def bwd_inputs(kind, B, H, Sq, Skv, visible, gen, device, softmax_scale=2.0 ** -4):
+    """q, k, v, o, dO (BSHD bf16) and lse (fp32 [B, H, Sq]) of one backward case (module docstring): "onehot", "uniform_q",
+    "uniform_k" (exact, bwd_exact_ref) or "random" (attention_bwd_bound; o and lse those of the forward)."""
+    seen = visible.any(-1)
+    dO = grid_bf16((B, Sq, H, 128), gen, device)
+    if kind == "random":
+        q, k, v = (rand_bf16((B, S, H, 128), gen, device) for S in (Sq, Skv, Skv))
+        dO = rand_bf16((B, Sq, H, 128), gen, device)
+        lse, o = lse_and_out(q, k, v, visible, softmax_scale)
+        return q, k, v, o, dO, lse
+    v = _few_channels((B, Skv, H, 128), gen, device)
+    o = _few_channels((B, Sq, H, 128), gen, device)
+    if kind == "onehot":
+        q, k, _ = onehot_qk(B, H, Sq, Skv, visible, gen, device)
+        top = float(torch.tensor(8192.0) * torch.tensor(scale_log2_f32(softmax_scale), dtype=torch.float32))
+    else:
+        q, k = grid_bf16((B, Sq, H, 128), gen, device), grid_bf16((B, Skv, H, 128), gen, device)
+        (q if kind == "uniform_q" else k).zero_()
+        top = 0.0
+    lse = torch.full((B, H, Sq), top, device=device).masked_fill(~seen, float("-inf"))
+    return q, k, v, o, dO, lse
+
+
+def _grid_quantum(t):
+    """The largest power of two that divides every element of t (fp64, finite)."""
+    t = t[t != 0]
+    for e in range(20, -140, -1):
+        if bool(((t * 2.0 ** -e) == (t * 2.0 ** -e).round()).all()):
+            return 2.0 ** e
+    raise AssertionError("no grid")
+
+
+def _exact_sum_ok(w, x, name):
+    """w [.., M, K] @ x [.., K, N] is exact in fp32 in any order: every product on one grid, magnitude sum below 2^24
+    quanta."""
+    x = x * (w != 0).any(-2)[..., None]  # only the rows of x that some product uses
+    if not bool((w != 0).any()) or not bool((x != 0).any()):
+        return
+    qnt = _grid_quantum(w) * _grid_quantum(x)
+    assert float((w.abs() @ x.abs()).max()) < 2.0 ** 24 * qnt, f"exact backward: {name} partial sums reach 2^24 quanta"
+
+
+def bwd_exact_ref(q, k, v, o, dO, lse, visible, softmax_scale):
+    """Exact dq, dk, dv (BSHD bf16) and delta (fp32 [B, H, Sq]) of the backward constructions (module docstring), and P
+    (fp64 [B, H, Sq, Skv], 0 or 1). Asserts the premises that make the kernels' arithmetic exact."""
+    qh, kh, vh, oh, gh = _bhsd64(q, k, v, o, dO)
+    lse64 = lse.double()[..., None]
+    assert not bool((visible & torch.isneginf(lse64)).any()), "a row with lse = -inf sees a key"
+    s = (qh @ kh.transpose(-1, -2)).masked_fill(~visible, 0)
+    assert bool((s == s.round()).all() and (s.abs() < 2 ** 24).all()), "exact backward needs integer logits"
+    sl = scale_log2_f32(softmax_scale)
+    x = (s * sl - torch.where(torch.isfinite(lse64), lse64, torch.zeros_like(lse64))).masked_fill(~visible, -1e9)
+    one = visible & (x == 0)
+    assert bool((one | (x <= -150)).all()), "exact backward: a visible logit is neither at lse nor 150 below it"
+    P = one.double()
+    dP = gh @ vh.transpose(-1, -2)
+    delta = (gh * oh).sum(-1)
+    d = (dP - delta[..., None]) * P
+    assert bool(((d * 256) == (d * 256).round()).all() and ((d * 256).abs() < 256).all()), \
+        "exact backward: dP - delta must be fewer than 256 quanta of 2^-8"
+    used = P.any(-1)
+    assert bool(((dP * P).float().double() == dP * P).all() and (delta[used].float().double() == delta[used]).all())
+    # the kernels' fp32 dS = (P (dP - delta)) scale, with torch fp32 ops
+    p32 = P.float()
+    ds32 = (p32 * (dP.float() - delta.float()[..., None])) * torch.full_like(p32, f32(softmax_scale))
+    dS = ds32.double()
+    assert bool((ds32.bfloat16().double() == dS).all()), "exact backward: bf16(dS) != dS"
+    for w, xx, name in ((P.transpose(-1, -2), gh, "dV"), (dS.transpose(-1, -2), qh, "dK"), (dS, kh, "dQ")):
+        _exact_sum_ok(w, xx, name)
+    out = lambda t: t.float().bfloat16().permute(0, 2, 1, 3)
+    return (out(dS @ kh), out(dS.transpose(-1, -2) @ qh), out(P.transpose(-1, -2) @ gh), delta.float(), P)
+
+
+def attention_bwd_bound(q, k, v, o, dO, lse, visible, softmax_scale, walk_q=None, walk_k=None):
+    """fp64 references and element bounds of dq, dk, dv (BSHD) and delta ([B, H, Sq]) on random inputs (module
+    docstring), against the kernel's formula on its inputs: lse (fp32) as passed, scale_log2 = fl(fl(scale) fl(log2 e)).
+    walk_q / walk_k: the q rows / keys the second GEMMs walk (default: S rounded up to 64). Returns
+    ((dq_ref, dq_bound), (dk_ref, dk_bound), (dv_ref, dv_bound), (delta_ref, delta_bound))."""
+    qh, kh, vh, oh, gh = _bhsd64(q, k, v, o, dO)
+    D, Sq, Skv = qh.shape[-1], qh.shape[2], kh.shape[2]
+    walk_q = walk_q or 64 * math.ceil(Sq / 64)
+    walk_k = walk_k or 64 * math.ceil(Skv / 64)
+    sl, sc = scale_log2_f32(softmax_scale), f32(softmax_scale)
+    lse64 = lse.double()[..., None]
+    assert not bool((visible & torch.isneginf(lse64)).any()), "a row with lse = -inf sees a key"
+    zero = torch.zeros((), dtype=torch.float64, device=qh.device)
+    vis = visible
+    s = qh @ kh.transpose(-1, -2)
+    es = acc_coeff(D) * (qh.abs() @ kh.abs().transpose(-1, -2))
+    x = torch.where(vis, s * sl - torch.where(torch.isfinite(lse64), lse64, zero), zero)
+    dx = sl * es + U32 * (x.abs() + sl * es)  # the QK^T chain, then fma's rounding
+    ex = torch.expm1(math.log(2) * dx)
+    rho = torch.where(vis, ex + 2.0 ** -22 * (1 + ex), zero)  # relative error of the fp32 P (exp2: 2^-22)
+    P = torch.where(vis, torch.exp2(x), zero)
+    eP0 = torch.where(vis, P * rho + 2.0 ** -126, zero)  # ftz / subnormal results: 2^-126 absolute
+    eP = torch.where(vis, eP0 + half_ulp_bf16(P + eP0), zero)  # bf16(P)
+    dP = gh @ vh.transpose(-1, -2)
+    edp = acc_coeff(D) * (gh.abs() @ vh.abs().transpose(-1, -2))
+    delta = (gh * oh).sum(-1)
+    edelta = D * U32 * (gh.abs() * oh.abs()).sum(-1)
+    d = dP - delta[..., None]
+    ed = edp + edelta[..., None]
+    ed = ed + U32 * (d.abs() + ed)  # fl(dP - delta)
+    Dm = d.abs() + ed
+    dS = P * d * sc
+    eS0 = sc * (eP0 * Dm + P * ed) + 2 * U32 * sc * (P + eP0) * Dm  # P's error, d's error, fl(P d), fl(. scale)
+    eS = torch.where(vis, eS0 + half_ulp_bf16(dS.abs() + eS0), zero)  # bf16(dS)
+
+    def second(w, ew, x, walk):
+        ref = w @ x
+        b = ew @ x.abs() + acc_coeff(walk) * ((w.abs() + ew) @ x.abs())
+        b = b + half_ulp_bf16(ref.abs() + b)  # the bf16 store
+        return ref.permute(0, 2, 1, 3), b.permute(0, 2, 1, 3)
+
+    return (second(dS, eS, kh, walk_k), second(dS.transpose(-1, -2), eS.transpose(-1, -2), qh, walk_q),
+            second(P.transpose(-1, -2), eP.transpose(-1, -2), gh, walk_q), (delta, edelta + 1e-300))
+
+
+def bwd_coords(idx):
+    """Element (b, row, h, col) of dq / dk / dv -> the CTA (128 owned rows), consumer warpgroup and 8-column group."""
+    b, r, h, c = (int(i) for i in idx)
+    return dict(b=b, row=r, h=h, col=c, cta=r // 128, warpgroup=(r % 128) // 64, col_group=c // 8)

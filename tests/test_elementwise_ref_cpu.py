@@ -248,3 +248,150 @@ def test_attention_checkers_reject_defects():
     bad = simulate_kernel(q, torch.roll(k, 1, 2), v, visible, 128 ** -0.5)[0]
     with pytest.raises(AssertionError):
         R.assert_within(bad, oref, ob, "neighbouring head's K")
+
+
+# ------------------------------------------------------------------------------------------------ attention backward
+def simulate_bwd(q, k, v, o, dO, lse, visible, scale, order=1, perturb=0, tile=64):
+    """The attention backward in fp32 the way the kernels tile it: S and dP in fp32 from exact dots, P = exp2(fma(s,
+    scale_log2, -lse)) with a relative perturbation of perturb * 2^-22 (ex2 is exact at 0), bf16 P and dS, and dV, dK, dQ
+    accumulated in fp32 one 64-row tile at a time, in ascending (order 1) or descending (order -1) walk order. Returns dq,
+    dk, dv (BSHD bf16) and delta (fp32 [B, H, Sq])."""
+    qh, kh, vh, oh, gh = (t.permute(0, 2, 1, 3).double() for t in (q, k, v, o, dO))
+    Sq, Skv = qh.shape[2], kh.shape[2]
+    sl = R.scale_log2_f32(scale)
+    delta = (gh * oh).sum(-1).float()
+    s = (qh @ kh.transpose(-1, -2)).float()
+    dp = (gh @ vh.transpose(-1, -2)).float()
+    x = (s.double() * sl - lse.double()[..., None]).float()  # fma: the exact product, one rounding
+    p = torch.exp2(x.double())
+    p = torch.where(x == 0, p, p * (1 + perturb * 2.0 ** -22)).float().masked_fill(~visible, 0)
+    ds = (p * (dp - delta[..., None])) * torch.full_like(p, R.f32(scale))
+    pb, dsb = p.bfloat16().double(), ds.bfloat16().double()
+    dq = torch.zeros(qh.shape, dtype=torch.float32)
+    dk = torch.zeros(kh.shape, dtype=torch.float32)
+    dv = torch.zeros(kh.shape, dtype=torch.float32)
+    for t in list(range(0, Sq, tile))[::order]:
+        r = slice(t, t + tile)
+        dv += (pb[:, :, r].transpose(-1, -2) @ gh[:, :, r]).float()
+        dk += (dsb[:, :, r].transpose(-1, -2) @ qh[:, :, r]).float()
+    for t in list(range(0, Skv, tile))[::order]:
+        c = slice(t, t + tile)
+        dq += (dsb[:, :, :, c] @ kh[:, :, c]).float()
+    out = lambda a: a.bfloat16().permute(0, 2, 1, 3)
+    return out(dq), out(dk), out(dv), delta
+
+
+BWD_EXACT = ["onehot", "uniform_q", "uniform_k"]
+
+
+def _bwd_case(kind, masks, seed, scale=2.0 ** -4):
+    B, H = 2, 3
+    g = _gen(seed)
+    Sq, Skv = (65, 257) if masks == "dense" else (320, 320)
+    visible = R.visible_mask(B, H, Sq, Skv, CPU) if masks == "dense" else _blocks_visible(B, H, Sq, Skv, g)
+    return R.bwd_inputs(kind, B, H, Sq, Skv, visible, g, CPU, scale), visible
+
+
+@pytest.mark.parametrize("kind", BWD_EXACT)
+@pytest.mark.parametrize("masks", ["dense", "blocks"])
+def test_bwd_constructions_match_the_tiled_simulation(kind, masks):
+    (q, k, v, o, dO, lse), visible = _bwd_case(kind, masks, 21)
+    dq, dk, dv, delta, P = R.bwd_exact_ref(q, k, v, o, dO, lse, visible, 2.0 ** -4)
+    if masks == "blocks":  # rows that see more than 128 keys, rows that see none
+        assert int(visible.sum(-1).max()) > 128 and bool((~visible.any(-1)).any())
+    for order in (1, -1):
+        for perturb in (1, -1):
+            sq, sk, sv, sd = simulate_bwd(q, k, v, o, dO, lse, visible, 2.0 ** -4, order, perturb)
+            for got, ref, name in ((sq, dq, "dq"), (sk, dk, "dk"), (sv, dv, "dv")):
+                R.assert_exact(got, ref, f"simulated {name}", where=R.bwd_coords)
+            assert torch.equal(sd, delta)
+    seen = visible.any(-1)
+    if kind == "onehot":  # exactly one key per row that sees any: dV_j sums dO over the rows that target j
+        assert torch.equal(P.sum(-1), seen.double())
+    else:  # every visible pair
+        assert torch.equal(P.bool(), visible)
+    nz = lambda t: bool((t != 0).any())
+    assert nz(dq) == (kind != "uniform_k") and nz(dk) == (kind != "uniform_q") and nz(dv)
+
+
+@pytest.mark.parametrize("scale", [2.0 ** -4, 128 ** -0.5])
+@pytest.mark.parametrize("masks", ["dense", "blocks"])
+def test_attention_bwd_bound_accepts_the_simulation(scale, masks):
+    (q, k, v, o, dO, lse), visible = _bwd_case("random", masks, 23, scale)
+    bounds = R.attention_bwd_bound(q, k, v, o, dO, lse, visible, scale)
+    for order in (1, -1):
+        for perturb in (1, -1):
+            sim = simulate_bwd(q, k, v, o, dO, lse, visible, scale, order, perturb)
+            for got, (ref, b), name in zip(sim, bounds, ("dq", "dk", "dv", "delta")):
+                R.assert_within(got, ref, b, f"simulated {name}", where=R.bwd_coords if name != "delta" else None)
+
+
+def _bwd_checker(kind, q, k, v, o, dO, lse, visible, scale):
+    """check(dq, dk, dv) against the exact reference (constructions) or the element bound (random)."""
+    if kind == "random":
+        refs = R.attention_bwd_bound(q, k, v, o, dO, lse, visible, scale)[:3]
+        return lambda *outs: [R.assert_within(t, r, b, n) for t, (r, b), n in zip(outs, refs, "qkv")]
+    refs = R.bwd_exact_ref(q, k, v, o, dO, lse, visible, scale)[:3]
+    return lambda *outs: [R.assert_exact(t, r, n) for t, r, n in zip(outs, refs, "qkv")]
+
+
+@pytest.mark.parametrize("kind", ["onehot", "uniform_q", "uniform_k", "random"])
+def test_attention_bwd_checkers_reject_defects(kind):
+    """Each defect, made by running the simulation on altered inputs or editing its output, fails the check of at least
+    the gradient it touches."""
+    B, H, Sq, Skv = 2, 3, 129, 192
+    g = _gen(31)
+    visible = R.visible_mask(B, H, Sq, Skv, CPU)
+    visible[:, :, :, 150:] = False  # a kv_len of 150: masked keys to count
+    scale = 2.0 ** -4
+    q, k, v, o, dO, lse = R.bwd_inputs(kind, B, H, Sq, Skv, visible, g, CPU, scale)
+    check = _bwd_checker(kind, q, k, v, o, dO, lse, visible, scale)
+    dq, dk, dv, _ = simulate_bwd(q, k, v, o, dO, lse, visible, scale)
+    check(dq, dk, dv)
+
+    def rejects(*outs):
+        with pytest.raises(AssertionError):
+            check(*outs)
+
+    def sim(vis=visible, l=lse):
+        return simulate_bwd(q, k, v, o, dO, l, vis, scale)
+
+    vis = visible.clone()
+    vis[1, 2, 64:128, 64:128] = False  # one 64-key tile missing from one dQ tile, one q tile from one dK / dV tile
+    mq, mk, mv, _ = sim(vis)
+    m = dq.clone()
+    m[1, 64:128, 2] = mq[1, 64:128, 2]
+    if kind != "uniform_k":
+        rejects(m, dk, dv)
+    m = dv.clone()
+    m[1, 64:128, 2] = mv[1, 64:128, 2]
+    rejects(dq, dk, m)
+    if kind != "uniform_q":
+        m = dk.clone()
+        m[1, 64:128, 2] = mk[1, 64:128, 2]
+        rejects(dq, m, dv)
+    # a row shifted by one, a head swapped, in the gradients the construction makes row- and head-dependent
+    for i, t in enumerate((dq, dk, dv)):
+        if not bool((t != 0).any()) or (kind.startswith("uniform") and i == 2):
+            continue  # uniform: every dv row of a head sums the same rows
+        outs = [dq, dk, dv]
+        shifted = t.clone()
+        shifted[1, 70] = t[1, 71]
+        outs[i] = shifted
+        rejects(*outs)
+        head = t.clone()
+        head[0, 64:128, 1] = t[0, 64:128, 2]
+        outs[i] = head
+        rejects(*outs)
+    if kind.startswith("uniform"):  # one masked key counted in one row
+        vis = visible.clone()
+        vis[1, 2, 100, 150] = True
+        mq, mk, mv, _ = sim(vis)
+        rejects(dq, dk, mv)
+        rejects(dq, mk, dv) if kind == "uniform_k" else rejects(mq, dk, dv)
+    if kind in ("onehot", "random"):  # an lse off by 0.25 in one row
+        l2 = lse.clone()
+        l2[0, 1, 40] += 0.25
+        mq, mk, mv, _ = sim(l=l2)
+        rejects(mq, dk, dv)
+        rejects(dq, dk, mv)

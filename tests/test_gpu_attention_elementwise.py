@@ -29,19 +29,6 @@ def _strides(t):
     return (c_int64 * 3)(t.stride(0), t.stride(1), t.stride(2))
 
 
-def make_qkv(B, Sq, Skv, H, layout):
-    """Uninitialised q [B, Sq, H, 128] and k, v [B, Skv, H, 128] views in one of three layouts."""
-    if layout == "bshd":
-        return (torch.empty(B, Sq, H, 128, dtype=torch.bfloat16, device=DEV),
-                *(torch.empty(B, Skv, H, 128, dtype=torch.bfloat16, device=DEV) for _ in range(2)))
-    if layout == "bhsd":
-        return (torch.empty(B, H, Sq, 128, dtype=torch.bfloat16, device=DEV).transpose(1, 2),
-                *(torch.empty(B, H, Skv, 128, dtype=torch.bfloat16, device=DEV).transpose(1, 2) for _ in range(2)))
-    qb = torch.empty(B, Sq, 3, H, 128, dtype=torch.bfloat16, device=DEV)  # fused [B, S, 3, H, 128] GEMM outputs
-    kvb = torch.empty(B, Skv, 3, H, 128, dtype=torch.bfloat16, device=DEV)
-    return qb[:, :, 0], kvb[:, :, 1], kvb[:, :, 2]
-
-
 class Outputs:
     """o in a [B, Sq + 2, H, 136] sentinel buffer (gaps between tokens and heads), LSE in a buffer with
     lse_stride_h = Sq + 8 and lse_stride_b = H (Sq + 8) + 16."""
@@ -83,21 +70,12 @@ def run(mode, q, k, v, out, scale, sel=None, q_off=None, q_len=None, kv_off=None
                                   c_int64(0 if sh_ == 1 else npairs), c_int(cap), c_int(npairs), i32p(q_off), i32p(q_len),
                                   c_int(nqb), i32p(kv_off), i32p(kv_len), c_int(nkb), sp()))
         return
-    idx, num = block_lists(sel)
+    idx, num = R.block_lists(sel)
     cap = idx.shape[-1]
     ws = torch.empty(256, dtype=torch.uint8, device=DEV)
     check(L.fvb_attention_blocklist_fwd(*common, i32p(idx), i32p(num), c_int64(0 if sb_ == 1 else sh_ * nqb),
                                         c_int64(0 if sh_ == 1 else nqb), c_int(cap), i32p(q_off), i32p(q_len), c_int(nqb),
                                         i32p(kv_off), i32p(kv_len), c_int(nkb), ptr(ws), c_int64(256), sp()))
-
-
-def block_lists(sel):
-    """bool [b, h, nqb, nkb] -> ascending lists int32 [b, h, nqb, nkb] (-1 padded) and counts [b, h, nqb]."""
-    num = sel.sum(-1).to(torch.int32)
-    key = torch.where(sel, torch.arange(sel.shape[-1], device=sel.device), sel.shape[-1])
-    idx = key.sort(-1).values.to(torch.int32)
-    idx[idx == sel.shape[-1]] = -1
-    return idx.contiguous(), num.contiguous()
 
 
 def pair_schedule(sel):
@@ -171,7 +149,7 @@ def test_dense(Sq, Skv):
     B, H = 2, 3
     i = DENSE.index((Sq, Skv))
     layout, scale = LAYOUTS[i % 3], (128 ** -0.5 if i % 2 == 0 else 0.0625)
-    q, k, v = make_qkv(B, Sq, Skv, H, layout)
+    q, k, v = R.make_qkv(B, Sq, Skv, H, layout, DEV)
     visible = R.visible_mask(B, H, Sq, Skv, DEV)
     g = torch.Generator(device=DEV).manual_seed(Sq * 1000 + Skv)
     for kind in ("uniform", "onehot", "random"):
@@ -183,7 +161,7 @@ def test_dense(Sq, Skv):
 
 def test_dense_checkers_reject_defects_on_kernel_output():
     B, H, Sq, Skv = 2, 3, 129, 128
-    q, k, v = make_qkv(B, Sq, Skv, H, "bshd")
+    q, k, v = R.make_qkv(B, Sq, Skv, H, "bshd", DEV)
     visible = R.visible_mask(B, H, Sq, Skv, DEV)
     g = torch.Generator(device=DEV).manual_seed(5)
     for kind in ("uniform", "onehot", "random"):
@@ -230,17 +208,6 @@ KV_LEN = [64, 0, 37, 64, 1, 50, 0]
 Q_LEN = [64, 30, 64, 1, 64, 63, 17]  # padded layout: rows past q_len keep their sentinels
 
 
-def _select(nqb, nkb, topk, bcast, g):
-    """bool [b, h, nqb, nkb] with topk blocks per q block; q block 3 selects only the empty kv blocks 1 and 6."""
-    b, h = {"none": (2, 3), "batch": (1, 3), "both": (1, 1)}[bcast]
-    sel = torch.zeros(b, h, nqb, nkb, dtype=torch.bool, device=DEV)
-    score = torch.rand(b, h, nqb, nkb, generator=g, device=DEV)
-    sel.scatter_(-1, score.topk(topk, -1).indices, True)
-    sel[:, :, 3] = False
-    sel[:, :, 3, [1, 6]] = True
-    return sel
-
-
 @pytest.mark.parametrize("mode", ["blocklist", "pairs"])
 @pytest.mark.parametrize("layout", ["padded", "compact"])
 @pytest.mark.parametrize("bcast", ["none", "batch", "both"])
@@ -268,9 +235,9 @@ def test_block_modes(mode, layout, bcast):
     # a fixed seed per case (str hashes change from one interpreter to the next): a failure replays with the same inputs
     g = torch.Generator(device=DEV).manual_seed(zlib.crc32(f"{mode}/{layout}/{bcast}".encode()))
     for kind, topk in (("uniform", 3), ("onehot", 3), ("random", 3)):
-        sel = _select(nqb, nkb, topk, bcast, g)
+        sel = R.select_blocks(nqb, nkb, topk, bcast, g, DEV)
         visible = R.visible_mask(B, H, Sq, Skv, DEV, q_block, kv_block, sel)
-        q, k, v = make_qkv(B, Sq, Skv, H, "bshd")
+        q, k, v = R.make_qkv(B, Sq, Skv, H, "bshd", DEV)
         fill(q, k, v, kind, visible, g)
         out = Outputs(B, Sq, H, seed=topk)
         out.mark_rows(written)
