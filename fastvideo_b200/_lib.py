@@ -35,6 +35,8 @@ def lib() -> ctypes.CDLL:
         _lib.fvb_resid_gate_bwd_workspace_bytes.restype = c_int64
         _lib.fvb_layernorm_modulate_bwd_workspace_bytes.restype = c_int64
         _lib.fvb_rmsnorm_rope_bwd_workspace_bytes.restype = c_int64
+        _lib.fvb_layernorm_modulate_grouped_bwd_workspace_bytes.restype = c_int64
+        _lib.fvb_resid_gate_grouped_bwd_workspace_bytes.restype = c_int64
     return _lib
 
 

@@ -33,7 +33,9 @@ import torch
 from . import ops
 from .distributed import out_proj_sp
 from .rope import get_rotary_pos_embed
-from .wan_dit import CrossAttnCache, Modulation, WanBlock, WanDiT, WanDiTConfig, block_tail, refuse_grad, refuse_model_grad
+from .wan_dit import (CrossAttnCache, Modulation, TokenLayout, WanBlock, WanDiT, WanDiTConfig, _HeadNormFramesFn,
+                      _any_model_tensor_requires_grad, _any_requires_grad, _linear, _require_trainable, _requires_grad,
+                      block_body, block_causal_tiles, block_forward_grad, block_tail, refuse_grad, refuse_model_grad)
 
 GLOBAL_ATTN_COMPAT_MAX_LATENT_FRAMES = 21  # causal_wanvideo.py:32
 
@@ -243,10 +245,20 @@ def _require_bf16_model(cfg: WanDiTConfig) -> None:
 
 
 def _pad_text(text: torch.Tensor, text_len: int) -> torch.Tensor:
-    """text padded with zero rows to text_len before the embedder (causal_wanvideo.py:604-609)."""
+    """text [B, L, text_dim] padded with zero rows to text_len before the embedder (causal_wanvideo.py:604-609)."""
     if text.shape[1] < text_len:
-        text = torch.cat([text, text.new_zeros(1, text_len - text.shape[1], text.shape[2])], 1)
+        text = torch.cat([text, text.new_zeros(text.shape[0], text_len - text.shape[1], text.shape[2])], 1)
     return text
+
+
+def causal_block_train(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb: torch.Tensor, lay: TokenLayout,
+                       cfg: WanDiTConfig, frame_seqlen: int, checkpoint: bool = False) -> torch.Tensor:
+    """The causal block of the training forward: x [S, D] bf16 (one sample, S = F * frame_seqlen), ctx [L, D], temb [F, 6, D]
+    bf16; block-causal self-attention over lay.causal, per-frame bf16 modulation. Differentiable (_WanBlockFn) when grad is
+    enabled and x, ctx, temb or a tensor of blk.tensors() requires grad; the plain block_body otherwise (the same bits)."""
+    if torch.is_grad_enabled() and _any_requires_grad(blk, x, ctx, temb):
+        return block_forward_grad(x, blk, ctx, Modulation.per_frame(blk, temb, frame_seqlen), lay, cfg, checkpoint)
+    return block_body(x, blk, ctx, Modulation.per_frame(blk, temb, frame_seqlen), lay, cfg)
 
 
 def _inference_only(path: str):
@@ -313,18 +325,64 @@ class CausalWanDiT(WanDiT):
 
     def forward(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor,
                 vsa_sparsity: float | None = None) -> torch.Tensor:
-        """WanDiT's bidirectional forward. Inference only for the causal model: its training (the block-causal mask, the
-        per-frame bf16 modulation backward) is not implemented, so it raises FvbError under grad with an input or a tensor
-        of tensors() requiring grad."""
+        """WanDiT's bidirectional forward. Inference only for the causal model (forward_train is its training forward): it
+        raises FvbError under grad with an input or a tensor of tensors() requiring grad."""
         refuse_model_grad("CausalWanDiT", self, latents, text)
         return super().forward(latents, text, timestep, vsa_sparsity)
+
+    def train_layout(self, seq_shape: tuple, start_frame: int, device) -> TokenLayout:
+        """Raster-order layout of the training forward: float64 RoPE tables at absolute frame positions from start_frame
+        (with fp32 copies for the RoPE backward) and the block-causal tile tables (wan_dit.block_causal_tiles)."""
+        F_, Hh, Ww = seq_shape
+        key = ("train", tuple(seq_shape), start_frame, str(device))
+        if key not in self._layouts:
+            cos, sin = self.rope_tables(F_, (Hh, Ww), start_frame, device)
+            tiles = block_causal_tiles(F_, Hh * Ww, self.ccfg.num_frames_per_block, self.ccfg.local_attn_size, device)
+            self._layouts[key] = TokenLayout(seq_shape=tuple(seq_shape), cos=cos, sin=sin, causal=tiles,
+                                             cos32=cos.float().contiguous(), sin32=sin.float().contiguous())
+        return self._layouts[key]
+
+    def forward_train(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor, start_frame: int = 0,
+                      checkpoint: bool = False) -> torch.Tensor:
+        """The training forward of the causal model (CausalWanTransformer3DModel._forward_train, causal_wanvideo.py:420-471):
+        latents [B, C, F, H, W] bf16, text [B, L, text_dim], timestep [B, F] (one per latent frame) -> flow prediction, same
+        shape as latents. Self-attention is block-causal: token i of frame block b (num_frames_per_block frames) attends the
+        keys before the end of its block, and with local_attn_size != -1 only the last local_attn_size frames of them.
+        Everything else is forward_inference's arithmetic (per-frame bf16 modulation, float64 RoPE at absolute positions from
+        start_frame, text padded to text_len, per-frame head). Differentiable in latents, text and every tensor of tensors()
+        when grad is enabled and one of them requires grad (the output has the bits of the call without grad). checkpoint:
+        under grad, each block keeps only its input, its modulation and its self-attention output and LSE."""
+        cfg = self.cfg
+        if _any_model_tensor_requires_grad(self, latents, text):  # refused before anything runs
+            if cfg.vsa:
+                raise ops.FvbError("the causal model has no sparse self-attention path: build it with vsa=False to train it")
+            for blk in self.blocks:
+                _require_trainable(blk, cfg)
+        if not latents.is_cuda:
+            raise ops.FvbError("CausalWanDiT.forward_train needs CUDA tensors (there is no CPU fallback)")
+        B = latents.shape[0]
+        pt, ph, pw = cfg.patch_size
+        F_, Hh, Ww = latents.shape[2] // pt, latents.shape[3] // ph, latents.shape[4] // pw
+        if tuple(timestep.shape) != (B, F_):
+            raise ops.FvbError(f"forward_train takes one timestep per latent frame: [{B}, {F_}], got {tuple(timestep.shape)}")
+        fs = Hh * Ww
+        lay = self.train_layout((F_, Hh, Ww), start_frame, latents.device)
+        temb, tproj, ctx = self.condition(timestep.flatten(), _pad_text(text, cfg.text_len))  # [B F, D], [B F, 6, D], [B, L, D]
+        x = self.patchify(latents.to(torch.bfloat16), lay)
+        outs = []
+        for b in range(B):
+            xb, frames = x[b], slice(b * F_, (b + 1) * F_)
+            for blk in self.blocks:
+                xb = causal_block_train(xb, blk, ctx[b], tproj[frames], lay, cfg, fs, checkpoint)
+            outs.append(self.head_per_frame(xb, temb[frames], fs))
+        return self.unpatchify(torch.stack(outs, 0), lay)
 
     @_inference_only("CausalWanDiT.forward_inference")
     def forward_inference(self, latents: torch.Tensor, text: torch.Tensor, timestep: torch.Tensor, kv_cache: list,
                           crossattn_cache: list | None, current_start: int = 0, start_frame: int = 0) -> torch.Tensor:
         """latents [1, C, F, H, W] bf16 (the frame block being denoised), text [1, L, text_dim] bf16, timestep [1, F]
         (one per latent frame). Returns the flow prediction [1, C, F, H, W]. Raises FvbError under grad with an input or a
-        tensor of tensors() requiring grad (there is no causal backward)."""
+        tensor of tensors() requiring grad (there is no backward through the KV-cache rollout; forward_train trains the model)."""
         cfg = self.cfg
         if not latents.is_cuda:
             raise ops.FvbError("CausalWanDiT.forward_inference needs CUDA tensors (there is no CPU fallback)")
@@ -353,8 +411,11 @@ class CausalWanDiT(WanDiT):
         if temb.dtype != torch.bfloat16 or self.scale_shift_table.dtype != torch.bfloat16:
             raise ops.FvbError("the causal head implements the bf16 modulation flow (bf16 temb and scale_shift_table)")
         e = (self.scale_shift_table.reshape(1, 2, D) + temb.unsqueeze(1)).float()  # [F, 2, D], bf16 values
-        n = ops.layernorm_modulate(x, e[:, 1], e[:, 0], round_ln=True, eps=self.cfg.eps, mod_rows=frame_seqlen, mod_bf16=True)
-        return ops.linear(n, self.w_out, self.b_out)
+        if _requires_grad(x, e):
+            n = _HeadNormFramesFn.apply(x, e[:, 1], e[:, 0], frame_seqlen, self.cfg.eps)
+        else:
+            n = ops.layernorm_modulate(x, e[:, 1], e[:, 0], round_ln=True, eps=self.cfg.eps, mod_rows=frame_seqlen, mod_bf16=True)
+        return _linear(n, self.w_out, self.b_out)
 
 
 # ----------------------------------------------------------------------------------------------------------------

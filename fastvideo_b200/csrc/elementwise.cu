@@ -991,6 +991,162 @@ __global__ void __launch_bounds__(EW_THREADS) layernorm_modulate_bwd_kernel(
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// Per-row-group (per latent frame) backward of the bf16 modulation flow (fvb_layernorm_modulate_grouped_bwd,
+// fvb_resid_gate_grouped_bwd; arithmetic in include/fvb200.h). Group g = rows [g R, min((g + 1) R, M)); `parts` CTAs per
+// group, CTA (g, p) = blockIdx.x = g * parts + p takes the group's rows p, p + parts, ... in row order, and writes its
+// fp32 column partials to part[blockIdx.x]. grouped_colsum_kernel adds a group's partials in p order: no atomics, the
+// summation order depends on (M, R, D) only.
+// ------------------------------------------------------------------------------------------
+static inline int grouped_parts(int M, int R, int budget) {
+  const int G = (M + R - 1) / R;
+  const int p = budget / G;
+  return p < 1 ? 1 : (p > R ? R : p);
+}
+
+template <bool GIN_F32>
+__global__ void __launch_bounds__(EW_THREADS) layernorm_modulate_grouped_bwd_kernel(
+    const __nv_bfloat16* __restrict__ x, int64_t ldx, const __nv_bfloat16* __restrict__ dn, int64_t lddn,
+    const float* __restrict__ scale, int mod_rows, int64_t mod_stride, const void* __restrict__ gin_, int64_t ldgin,
+    __nv_bfloat16* __restrict__ dx, int64_t lddx, float* __restrict__ part, int M, int D, float eps, int parts) {
+  __shared__ float red[32];
+  __shared__ float2 red2[32];
+  const int g = blockIdx.x / parts, p = blockIdx.x - g * parts;
+  const int64_t r1 = min(int64_t(g + 1) * mod_rows, int64_t(M));
+  scale += int64_t(g) * mod_stride;
+  const int nchunks = D >> 3;
+  float as[EW_MAX_CHUNKS][8], ah[EW_MAX_CHUNKS][8];
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) as[c][i] = ah[c][i] = 0.f;
+  for (int64_t row = int64_t(g) * mod_rows + p; row < r1; row += parts) {
+    float xv[EW_MAX_CHUNKS][8], dv[EW_MAX_CHUNKS][8];
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        unpack8(*reinterpret_cast<const uint4*>(x + row * ldx + (ch << 3)), xv[c]);
+        unpack8(*reinterpret_cast<const uint4*>(dn + row * lddn + (ch << 3)), dv[c]);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s += xv[c][i];
+      }
+    }
+    const float mean = block_sum(s, red) / float(D);
+    float q = 0.f;
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float d = xv[c][i] - mean;
+          q += d * d;
+        }
+    }
+    const float rstd = rsqrtf(block_sum(q, red) / float(D) + eps);
+    float2 st = make_float2(0.f, 0.f);  // (sum dt, sum dt * xhat)
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        float sc[8];
+        load8_f32(scale + (ch << 3), sc);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float xh = (xv[c][i] - mean) * rstd;  // the forward's LN output before its bf16 rounding
+          xv[c][i] = xh;
+          // dv becomes dt = bf16(dn * bf16(1 + scale)) once dn has gone into the group sums
+          as[c][i] = __fmaf_rn(dv[c][i], bf16_round(xh), as[c][i]);
+          ah[c][i] = __fadd_rn(ah[c][i], dv[c][i]);
+          dv[c][i] = bf16_round(__fmul_rn(dv[c][i], bf16_round(__fadd_rn(1.0f, sc[i]))));
+          st.x += dv[c][i];
+          st.y = __fmaf_rn(dv[c][i], xh, st.y);
+        }
+      }
+    }
+    st = block_sum2(st, red2);
+    const float mdt = __fdiv_rn(st.x, float(D)), mdx = __fdiv_rn(st.y, float(D));
+#pragma unroll
+    for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+      const int ch = threadIdx.x + c * EW_THREADS;
+      if (ch < nchunks) {
+        float o[8], gi[8];
+        if (gin_ != nullptr) {
+          if constexpr (GIN_F32)
+            load8_f32(reinterpret_cast<const float*>(gin_) + row * ldgin + (ch << 3), gi);
+          else
+            unpack8(*reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(gin_) + row * ldgin + (ch << 3)), gi);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          o[i] = __fmul_rn(rstd, __fsub_rn(__fsub_rn(dv[c][i], mdt), __fmul_rn(xv[c][i], mdx)));
+          if (gin_ != nullptr) o[i] = __fadd_rn(o[i], gi[i]);
+        }
+        *reinterpret_cast<uint4*>(dx + row * lddx + (ch << 3)) = pack8(o);
+      }
+    }
+  }
+  const int64_t nblk = gridDim.x;
+#pragma unroll
+  for (int c = 0; c < EW_MAX_CHUNKS; ++c) {
+    const int ch = threadIdx.x + c * EW_THREADS;
+    if (ch < nchunks) {
+      float4* ds = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * D + (ch << 3));
+      float4* dh = reinterpret_cast<float4*>(part + (nblk + blockIdx.x) * D + (ch << 3));
+      ds[0] = make_float4(as[c][0], as[c][1], as[c][2], as[c][3]);
+      ds[1] = make_float4(as[c][4], as[c][5], as[c][6], as[c][7]);
+      dh[0] = make_float4(ah[c][0], ah[c][1], ah[c][2], ah[c][3]);
+      dh[1] = make_float4(ah[c][4], ah[c][5], ah[c][6], ah[c][7]);
+    }
+  }
+}
+
+// The layout of resid_gate_bwd_kernel (blockIdx.y picks 1024 columns, 8 per thread) with blockIdx.x = g * parts + p as above.
+__global__ void __launch_bounds__(BG_THREADS) resid_gate_grouped_bwd_kernel(
+    const __nv_bfloat16* __restrict__ dout, int64_t lddout, const __nv_bfloat16* __restrict__ y, int64_t ldy,
+    const float* __restrict__ gate, int gate_rows, int64_t gate_stride, __nv_bfloat16* __restrict__ dy, int64_t lddy,
+    float* __restrict__ part, int M, int N, int parts) {
+  const int col = (blockIdx.y * BG_THREADS + threadIdx.x) * 8;
+  if (col >= N) return;
+  const int g = blockIdx.x / parts, p = blockIdx.x - g * parts;
+  const int64_t r1 = min(int64_t(g + 1) * gate_rows, int64_t(M));
+  float gv[8], ag[8], ab[8];
+  load8_f32(gate + int64_t(g) * gate_stride + col, gv);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) ag[i] = ab[i] = 0.f;
+  for (int64_t row = int64_t(g) * gate_rows + p; row < r1; row += parts) {
+    float d[8], yv[8], o[8];
+    unpack8(*reinterpret_cast<const uint4*>(dout + row * lddout + col), d);
+    unpack8(*reinterpret_cast<const uint4*>(y + row * ldy + col), yv);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[i] = bf16_round(__fmul_rn(d[i], gv[i]));
+      ag[i] = __fmaf_rn(d[i], yv[i], ag[i]);
+      ab[i] = __fadd_rn(ab[i], o[i]);
+    }
+    *reinterpret_cast<uint4*>(dy + row * lddy + col) = pack8(o);
+  }
+  float4* dg = reinterpret_cast<float4*>(part + int64_t(blockIdx.x) * N + col);
+  float4* db = reinterpret_cast<float4*>(part + (int64_t(gridDim.x) + blockIdx.x) * N + col);
+  dg[0] = make_float4(ag[0], ag[1], ag[2], ag[3]);
+  dg[1] = make_float4(ag[4], ag[5], ag[6], ag[7]);
+  db[0] = make_float4(ab[0], ab[1], ab[2], ab[3]);
+  db[1] = make_float4(ab[4], ab[5], ab[6], ab[7]);
+}
+
+// out[g * ldo + col] = sum over p (in order) of part[(g * parts + p) * N + col]; blockIdx.y = g
+__global__ void __launch_bounds__(256) grouped_colsum_kernel(const float* __restrict__ part, int parts, int N,
+                                                             float* __restrict__ out, int64_t ldo) {
+  const int col = blockIdx.x * 256 + threadIdx.x;
+  if (col >= N) return;
+  const float* src = part + int64_t(blockIdx.y) * parts * N + col;
+  float s = 0.f;
+  for (int i = 0; i < parts; ++i) s = __fadd_rn(s, __ldg(src + int64_t(i) * N));
+  out[int64_t(blockIdx.y) * ldo + col] = s;
+}
+
 }  // namespace fvb
 
 using namespace fvb;
@@ -1290,5 +1446,79 @@ extern "C" int fvb_layernorm_modulate_bwd(const void* x, int x_is_f32, int64_t l
   FVB_CHECK_CUDA(cudaGetLastError());
   colsum_f32_kernel<<<(D + 255) / 256, 256, 0, st>>>(workspace + int64_t(ctas) * D, ctas, D, d_offset);
   FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_layernorm_modulate_grouped_bwd_workspace_bytes(int M, int mod_rows, int D) {
+  if (M <= 0 || mod_rows <= 0 || D <= 0) return 0;
+  const int64_t G = (M + mod_rows - 1) / mod_rows;
+  return 2 * G * grouped_parts(M, mod_rows, RB_CTAS) * int64_t(D) * int64_t(sizeof(float));
+}
+
+extern "C" int fvb_layernorm_modulate_grouped_bwd(const void* x, int64_t ldx, const void* dn, int64_t lddn, const float* scale,
+                                                  int mod_rows, int64_t mod_stride, const void* gin, int gin_is_f32,
+                                                  int64_t ldgin, void* dx, int64_t lddx, float* d_scale, float* d_shift,
+                                                  int64_t ld_dmod, float* workspace, int64_t workspace_bytes, int M, int D,
+                                                  float eps, void* stream) {
+  FVB_CHECK_ARG(x && dn && scale && dx && d_scale && d_shift && workspace, "null pointer");
+  FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
+  FVB_CHECK_ARG(mod_rows > 0 && mod_stride % 4 == 0 && mod_stride >= D, "bad modulation grouping (rows > 0, stride >= D and a multiple of 4)");
+  FVB_CHECK_ARG(ldx % 8 == 0 && lddn % 8 == 0 && lddx % 8 == 0 && (gin == nullptr || ldgin % 8 == 0), "strides must be multiples of 8");
+  FVB_CHECK_ARG(ld_dmod >= D, "ld_dmod must be >= D");
+  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(scale) & 15) == 0, "scale must be 16-byte aligned");
+  FVB_CHECK_ARG(workspace_bytes >= fvb_layernorm_modulate_grouped_bwd_workspace_bytes(M, mod_rows, D), "workspace too small");
+  const int G = (M + mod_rows - 1) / mod_rows;
+  const int parts = grouped_parts(M, mod_rows, RB_CTAS);
+  const int ctas = G * parts;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  auto* xb = reinterpret_cast<const __nv_bfloat16*>(x);
+  auto* dnb = reinterpret_cast<const __nv_bfloat16*>(dn);
+  auto* dxb = reinterpret_cast<__nv_bfloat16*>(dx);
+  if (gin_is_f32)
+    layernorm_modulate_grouped_bwd_kernel<true><<<ctas, EW_THREADS, 0, st>>>(xb, ldx, dnb, lddn, scale, mod_rows, mod_stride, gin,
+                                                                             ldgin, dxb, lddx, workspace, M, D, eps, parts);
+  else
+    layernorm_modulate_grouped_bwd_kernel<false><<<ctas, EW_THREADS, 0, st>>>(xb, ldx, dnb, lddn, scale, mod_rows, mod_stride, gin,
+                                                                              ldgin, dxb, lddx, workspace, M, D, eps, parts);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  const dim3 cgrid((D + 255) / 256, G);
+  grouped_colsum_kernel<<<cgrid, 256, 0, st>>>(workspace, parts, D, d_scale, ld_dmod);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  grouped_colsum_kernel<<<cgrid, 256, 0, st>>>(workspace + int64_t(ctas) * D, parts, D, d_shift, ld_dmod);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  return FVB_OK;
+}
+
+extern "C" int64_t fvb_resid_gate_grouped_bwd_workspace_bytes(int M, int gate_rows, int N) {
+  if (M <= 0 || gate_rows <= 0 || N <= 0) return 0;
+  const int64_t G = (M + gate_rows - 1) / gate_rows;
+  return 2 * G * grouped_parts(M, gate_rows, BG_PARTS) * int64_t(N) * int64_t(sizeof(float));
+}
+
+extern "C" int fvb_resid_gate_grouped_bwd(const void* dout, int64_t lddout, const void* y, int64_t ldy, const float* gate,
+                                          int gate_rows, int64_t gate_stride, void* dy, int64_t lddy, float* d_gate,
+                                          int64_t ld_dgate, void* db, float* workspace, int64_t workspace_bytes, int M, int N,
+                                          void* stream) {
+  FVB_CHECK_ARG(dout && y && gate && dy && d_gate && workspace, "null pointer");
+  FVB_CHECK_ARG(M > 0 && N > 0 && N % 8 == 0, "N must be a positive multiple of 8");
+  FVB_CHECK_ARG(gate_rows > 0 && gate_stride % 4 == 0 && gate_stride >= N, "bad gate grouping (rows > 0, stride >= N and a multiple of 4)");
+  FVB_CHECK_ARG(lddout % 8 == 0 && ldy % 8 == 0 && lddy % 8 == 0, "strides must keep rows 16-byte aligned");
+  FVB_CHECK_ARG(ld_dgate >= N, "ld_dgate must be >= N");
+  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gate) & 15) == 0, "gate must be 16-byte aligned");
+  FVB_CHECK_ARG(workspace_bytes >= fvb_resid_gate_grouped_bwd_workspace_bytes(M, gate_rows, N), "workspace too small");
+  const int G = (M + gate_rows - 1) / gate_rows;
+  const int parts = grouped_parts(M, gate_rows, BG_PARTS);
+  const int ctas = G * parts;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  resid_gate_grouped_bwd_kernel<<<dim3(ctas, (N / 8 + BG_THREADS - 1) / BG_THREADS), BG_THREADS, 0, st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(dout), lddout, reinterpret_cast<const __nv_bfloat16*>(y), ldy, gate, gate_rows,
+      gate_stride, reinterpret_cast<__nv_bfloat16*>(dy), lddy, workspace, M, N, parts);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  grouped_colsum_kernel<<<dim3((N + 255) / 256, G), 256, 0, st>>>(workspace, parts, N, d_gate, ld_dgate);
+  FVB_CHECK_CUDA(cudaGetLastError());
+  if (db != nullptr) {  // every group's partials, in (g, p) order
+    rmsnorm_bwd_dw_kernel<<<(N + 255) / 256, 256, 0, st>>>(workspace + int64_t(ctas) * N, ctas, N, reinterpret_cast<__nv_bfloat16*>(db));
+    FVB_CHECK_CUDA(cudaGetLastError());
+  }
   return FVB_OK;
 }

@@ -270,8 +270,10 @@ static int dispatch_epi_aux(int epi, const CUtensorMap& a, const CUtensorMap& b,
     case FVB_EPI_BIAS_GELU_TANH: return launch_gemm_aux<BN, FVB_EPI_BIAS_GELU_TANH>(a, b, p, st);
     case FVB_EPI_RESID_GATE_F32: return launch_gemm_aux<BN, FVB_EPI_RESID_GATE_F32>(a, b, p, st);
     case FVB_EPI_RESID_GATE_BF16: return launch_gemm_aux<BN, FVB_EPI_RESID_GATE_BF16>(a, b, p, st);
+    case FVB_EPI_RESID_GATE_BF16R: return launch_gemm_aux<BN, FVB_EPI_RESID_GATE_BF16R>(a, b, p, st);
   }
-  return set_error(FVB_ERR_INVALID_ARG, "fvb_linear_bf16_aux takes FVB_EPI_BIAS_GELU_TANH, _RESID_GATE_F32 or _RESID_GATE_BF16%s");
+  return set_error(FVB_ERR_INVALID_ARG,
+                   "fvb_linear_bf16_aux takes FVB_EPI_BIAS_GELU_TANH, _RESID_GATE_F32, _RESID_GATE_BF16 or _RESID_GATE_BF16R%s");
 }
 
 // fp8 / int8 operands: the public linear epilogues only (DIV / SCALE_F32 belong to bf16-only entry points)

@@ -118,11 +118,12 @@ def _check_2d(t: torch.Tensor, name: str, shape, dtypes=(torch.bfloat16,)) -> No
 
 def linear_aux(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, epilogue: int,
                resid: torch.Tensor | None = None, gate: torch.Tensor | None = None, gate_rows: int = 0):
-    """fvb_linear_bf16_aux: `linear` (bf16 weight, EPI_BIAS_GELU_TANH / EPI_RESID_GATE_F32 / EPI_RESID_GATE_BF16) that also
-    returns the bf16 y = bf16(x @ w.T + bias) its epilogue consumes. x: [M, K] with unit inner stride; one gate vector
-    (gate_rows 0). Returns (out, aux); out has the bits of `linear`, aux those of `linear` with EPI_BIAS."""
-    if gate_rows != 0:
-        raise FvbError("linear_aux takes one gate vector for all rows (gate_rows=0)")
+    """fvb_linear_bf16_aux: `linear` (bf16 weight, EPI_BIAS_GELU_TANH / EPI_RESID_GATE_F32 / EPI_RESID_GATE_BF16 /
+    EPI_RESID_GATE_BF16R) that also returns the bf16 y = bf16(x @ w.T + bias) its epilogue consumes. x: [M, K] with unit
+    inner stride; one gate vector (gate_rows 0), or [G, N] with gate_rows > 0 for EPI_RESID_GATE_BF16R. Returns (out, aux);
+    out has the bits of `linear`, aux those of `linear` with EPI_BIAS."""
+    if gate_rows != 0 and epilogue != EPI_RESID_GATE_BF16R:
+        raise FvbError("linear_aux takes per-row-group gates (gate_rows > 0) with EPI_RESID_GATE_BF16R only")
     _require_cuda_bf16(x, "x")
     _require_cuda_bf16(w, "w")
     if x.dim() != 2 or x.stride(1) != 1 or w.stride(1) != 1:
@@ -133,13 +134,13 @@ def linear_aux(x: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None, epil
     aux = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
     if resid is not None:
         _check_2d(resid, "resid", (M, N))
-    gate_stride = _check_grouped(gate, N, 0, M, "gate")
+    gate_stride = _check_grouped(gate, N, gate_rows, M, "gate")
     if bias is not None:
         _require_cuda_bf16(bias, "bias")
         assert bias.is_contiguous() and bias.numel() == N
     check(lib().fvb_linear_bf16_aux(ptr(x), c_int64(x.stride(0)), ptr(w), c_int64(w.stride(0)), ptr(bias), ptr(out),
                                     c_int64(N), ptr(resid), c_int64(resid.stride(0) if resid is not None else 0), _f32p(gate),
-                                    c_int(0), c_int64(gate_stride), ptr(aux), c_int64(N), c_int(M), c_int(N), c_int(K),
+                                    c_int(gate_rows), c_int64(gate_stride), ptr(aux), c_int64(N), c_int(M), c_int(N), c_int(K),
                                     c_int(epilogue), stream_ptr()))
     return out, aux
 
@@ -207,6 +208,60 @@ def layernorm_modulate_bwd(x: torch.Tensor, dn: torch.Tensor, scale: torch.Tenso
                                            _f32p(d_off), _f32p(ws), c_int64(ws.numel()), c_int(M), c_int(D), c_float(eps),
                                            stream_ptr()))
     return dx, d_gain, d_off
+
+
+def _check_groups(t: torch.Tensor, name: str, D: int, G: int) -> None:
+    if t.dtype != torch.float32 or t.dim() != 2 or t.shape != (G, D) or t.stride(1) != 1 or t.data_ptr() % 16:
+        raise FvbError(f"{name} must be an fp32 [{G}, {D}] view with unit inner stride, 16-byte aligned")
+
+
+def layernorm_modulate_grouped_bwd(x: torch.Tensor, dn: torch.Tensor, scale: torch.Tensor, mod_rows: int,
+                                   gin: torch.Tensor | None = None, eps: float = 1e-6):
+    """fvb_layernorm_modulate_grouped_bwd: backward of layernorm_modulate(x, scale, shift, round_ln=True, mod_rows=R,
+    mod_bf16=True) (one modulation row per group of R rows, bf16 arithmetic). x, dn bf16 [M, D]; scale fp32 [G, D] (G =
+    ceil(M / R); any row stride that is a multiple of 4, e.g. a slice of the [F, 6, D] modulation); gin: optional fp32 /
+    bf16 [M, D] gradient added into dx. Returns (dx bf16 [M, D], d_scale fp32 [G, D], d_shift fp32 [G, D])."""
+    M, D = x.shape
+    _check_2d(x, "x", (M, D))
+    _check_2d(dn, "dn", (M, D))
+    if mod_rows <= 0:
+        raise FvbError("layernorm_modulate_grouped_bwd: mod_rows must be > 0")
+    G = -(-M // mod_rows)
+    _check_groups(scale, "scale", D, G)
+    if gin is not None:
+        _check_2d(gin, "gin", (M, D), (torch.float32, torch.bfloat16))
+    dx = torch.empty((M, D), dtype=torch.bfloat16, device=x.device)
+    d_scale = torch.empty((G, D), dtype=torch.float32, device=x.device)
+    d_shift = torch.empty((G, D), dtype=torch.float32, device=x.device)
+    ws = _workspace(int(lib().fvb_layernorm_modulate_grouped_bwd_workspace_bytes(c_int(M), c_int(mod_rows), c_int(D))), x.device)
+    check(lib().fvb_layernorm_modulate_grouped_bwd(ptr(x), c_int64(x.stride(0)), ptr(dn), c_int64(dn.stride(0)), _f32p(scale),
+                                                   c_int(mod_rows), c_int64(scale.stride(0)), ptr(gin),
+                                                   c_int(int(gin is not None and gin.dtype == torch.float32)),
+                                                   c_int64(gin.stride(0) if gin is not None else 0), ptr(dx), c_int64(D),
+                                                   _f32p(d_scale), _f32p(d_shift), c_int64(D), _f32p(ws), c_int64(ws.numel()),
+                                                   c_int(M), c_int(D), c_float(eps), stream_ptr()))
+    return dx, d_scale, d_shift
+
+
+def resid_gate_grouped_bwd(dout: torch.Tensor, y: torch.Tensor, gate: torch.Tensor, gate_rows: int, need_db: bool = True):
+    """fvb_resid_gate_grouped_bwd: backward of out = bf16(resid + bf16(y * gate[r // gate_rows])) (EPI_RESID_GATE_BF16R with
+    gate_rows > 0). dout, y bf16 [M, N] (2-D views, unit inner stride), gate fp32 [G, N] (row stride a multiple of 4).
+    Returns (dy bf16 [M, N], d_gate fp32 [G, N], db bf16 [N] or None); the residual's gradient is dout."""
+    M, N = y.shape
+    _check_2d(dout, "dout", (M, N))
+    _check_2d(y, "y", (M, N))
+    if gate_rows <= 0:
+        raise FvbError("resid_gate_grouped_bwd: gate_rows must be > 0")
+    G = -(-M // gate_rows)
+    _check_groups(gate, "gate", N, G)
+    dy = torch.empty((M, N), dtype=torch.bfloat16, device=y.device)
+    d_gate = torch.empty((G, N), dtype=torch.float32, device=y.device)
+    db = torch.empty(N, dtype=torch.bfloat16, device=y.device) if need_db else None
+    ws = _workspace(int(lib().fvb_resid_gate_grouped_bwd_workspace_bytes(c_int(M), c_int(gate_rows), c_int(N))), y.device)
+    check(lib().fvb_resid_gate_grouped_bwd(ptr(dout), c_int64(dout.stride(0)), ptr(y), c_int64(y.stride(0)), _f32p(gate),
+                                           c_int(gate_rows), c_int64(gate.stride(0)), ptr(dy), c_int64(N), _f32p(d_gate),
+                                           c_int64(N), ptr(db), _f32p(ws), c_int64(ws.numel()), c_int(M), c_int(N), stream_ptr()))
+    return dy, d_gate, db
 
 
 def rmsnorm_rope_bwd(x0, w0, dy0, dx0, x1, w1, dy1, dx1, cos, sin, rope_row=None, head_dim: int = 128, eps: float = 1e-6,

@@ -223,6 +223,66 @@ class TokenLayout:
     block_off: torch.Tensor | None = None  # int32 [n_tiles + 1]
     row_block: torch.Tensor | None = None  # int32 [S] token position -> tile
     topk: int = 0
+    causal: "BlockCausalTiles | None" = None  # block-causal self-attention (causal model training)
+    cos32: torch.Tensor | None = None   # fp32 copies of float64 cos / sin for the RoPE backward (None: cos / sin are fp32)
+    sin32: torch.Tensor | None = None
+
+
+@dataclass
+class BlockCausalTiles:
+    """Block-causal self-attention as a block list over variable-length tiles (ops.attention_blocklist /
+    ops.attention_sparse_bwd). Token i of frame block b = i // (n fs) attends key j iff j < end_b = min((b + 1) n fs, S) and,
+    with a local window of W = local_attn_size fs tokens, j >= end_b - W. q tiles (at most 64 rows, token order) are cut at
+    every end_b, kv tiles also at every window start inside the sequence, so each (q tile, kv tile) pair is wholly inside or
+    wholly outside the mask."""
+    q_off: torch.Tensor     # int32 [nqb + 1]
+    kv_off: torch.Tensor    # int32 [nkb + 1]
+    tile_map: torch.Tensor  # bool [1, 1, nqb, nkb]
+    q2k_idx: torch.Tensor   # int32 [1, 1, nqb, nkb] / q2k_num [1, 1, nqb]: ops.map_to_index(tile_map)
+    q2k_num: torch.Tensor
+    k2q_idx: torch.Tensor   # int32 [1, 1, nkb, nqb] / k2q_num [1, 1, nkb]: the transposed map's lists
+    k2q_num: torch.Tensor
+
+    @property
+    def nkb(self) -> int:
+        return self.kv_off.numel() - 1
+
+
+def block_causal_tile_map(frames: int, frame_seqlen: int, frames_per_block: int, local_attn_size: int = -1):
+    """Host tile tables of the block-causal mask (BlockCausalTiles): (q_off int32 [nqb + 1], kv_off int32 [nkb + 1], tile_map
+    bool [nqb, nkb]). frames need not be a multiple of frames_per_block (the last block is shorter)."""
+    S, L = frames * frame_seqlen, frames_per_block * frame_seqlen
+    if S <= 0 or L <= 0 or (local_attn_size != -1 and local_attn_size <= 0):
+        raise ops.FvbError("block-causal tiles need frames, frame_seqlen, frames_per_block > 0 and local_attn_size -1 or > 0")
+    ends = [min(e, S) for e in range(L, S + L, L)]
+    W = local_attn_size * frame_seqlen if local_attn_size != -1 else None
+    lo = [max(0, e - W) if W is not None else 0 for e in ends]
+
+    def tiles(cuts):
+        cuts = sorted(set(cuts) | {0, S})
+        off = [a + i for a, b in zip(cuts, cuts[1:]) for i in range(0, b - a, 64)]
+        return torch.tensor(off + [S], dtype=torch.int32)
+
+    q_off, kv_off = tiles(ends), tiles(ends + lo)
+    block = torch.bucketize(q_off[:-1].long(), torch.tensor(ends), right=True)  # frame block of each q tile
+    end_q, lo_q = torch.tensor(ends)[block], torch.tensor(lo)[block]
+    tile_map = (kv_off[None, 1:].long() <= end_q[:, None]) & (kv_off[None, :-1].long() >= lo_q[:, None])
+    return q_off, kv_off, tile_map
+
+
+_BLOCK_CAUSAL: dict = {}
+
+
+def block_causal_tiles(frames: int, frame_seqlen: int, frames_per_block: int, local_attn_size: int, device) -> BlockCausalTiles:
+    """BlockCausalTiles on `device`, built once per (frames, frame_seqlen, frames_per_block, local_attn_size, device)."""
+    key = (frames, frame_seqlen, frames_per_block, local_attn_size, str(device))
+    if key not in _BLOCK_CAUSAL:
+        q_off, kv_off, tile_map = block_causal_tile_map(frames, frame_seqlen, frames_per_block, local_attn_size)
+        m = tile_map.to(device)[None, None]
+        q2k_idx, q2k_num = ops.map_to_index(m.contiguous())
+        k2q_idx, k2q_num = ops.map_to_index(m.transpose(-1, -2).contiguous())
+        _BLOCK_CAUSAL[key] = BlockCausalTiles(q_off.to(device), kv_off.to(device), m, q2k_idx, q2k_num, k2q_idx, k2q_num)
+    return _BLOCK_CAUSAL[key]
 
 
 def make_layout(seq_shape, cfg: WanDiTConfig, device, vsa_sparsity: float | None = None) -> TokenLayout:
@@ -376,14 +436,17 @@ def block_forward(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, temb6: torc
     checkpoint: under grad, keep only the block input, the modulation and the self-attention results
     (checkpoint_bytes_per_block); the backward re-runs the block around the saved self-attention first."""
     if torch.is_grad_enabled() and _any_requires_grad(blk, x, ctx, temb6):
-        return _block_forward_grad(x, blk, ctx, temb6, lay, cfg, checkpoint)
+        _require_trainable(blk, cfg)
+        # torch ops: autograd carries the six vectors back to scale_shift_table and temb6
+        return block_forward_grad(x, blk, ctx, Modulation.fp32(blk, temb6), lay, cfg, checkpoint)
     return block_body(x, blk, ctx, Modulation.fp32(blk, temb6), lay, cfg)
 
 
 def block_body(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulation, lay: TokenLayout, cfg: WanDiTConfig,
                keep: dict | None = None, attn: dict | None = None, replay: bool = False) -> torch.Tensor:
-    """The single-rank block: self-attention (wanvideo.py:393-415), then block_tail. `keep`: see _keep. `attn` (the
-    checkpointed block, _WanBlockFn) records the self-attention results: dense "a" and "lse"; VSA the tensors
+    """The single-rank block: self-attention (wanvideo.py:393-415; block-causal over lay.causal's tile lists when it is set),
+    then block_tail. `keep`: see _keep. `attn` (the checkpointed block, _WanBlockFn) records the self-attention results:
+    dense and block-causal "a" and "lse"; VSA the tensors
     _VideoSparseAttnFn saves besides q / k / v / gate, under their _VideoSparseAttnFn.SAVED names. With `replay` those
     results are used instead of launching the self-attention (for VSA the output is recombined from the saved branches
     and the recomputed gate by the same fvb_vsa_combine call, so the same bits)."""
@@ -416,6 +479,14 @@ def block_body(x: torch.Tensor, blk: WanBlock, ctx: torch.Tensor, mod: Modulatio
     elif replay:
         a = attn["a"]
         _keep(keep, lse=attn["lse"])
+    elif lay.causal is not None:  # block-causal (causal model training): the tile lists of lay.causal
+        c = lay.causal
+        a, lse = ops.attention_blocklist(q, k, v, c.q2k_idx, c.q2k_num, softmax_scale=d ** -0.5, return_lse=True,
+                                         q_off=c.q_off, kv_off=c.kv_off, nkb=c.nkb)
+        a = a.reshape(S, D)
+        _keep(keep, lse=lse)
+        if attn is not None:
+            attn.update(a=a, lse=lse)
     elif attn is not None:
         a, attn["lse"] = ops.attention(q, k, v, softmax_scale=d ** -0.5, return_lse=True)
         attn["a"] = a = a.reshape(S, D)
@@ -444,7 +515,7 @@ def refuse_grad(path: str, blk: WanBlock, *inputs) -> None:
 
 _BLOCK_TENSORS = ("w_qkv", "b_qkv", "norm_q", "norm_k", "w_o", "b_o", "norm2_w", "norm2_b", "w_q2", "b_q2", "w_kv2", "b_kv2",
                   "norm_q2", "norm_k2", "w_o2", "b_o2", "w_1", "b_1", "w_2", "b_2", "w_kv_img", "b_kv_img", "norm_k_img")
-_FN_LEAD = 12  # _WanBlockFn inputs before the block tensors: x, ctx, six modulation vectors, blk, lay, cfg, checkpoint
+_FN_LEAD = 13  # _WanBlockFn inputs before the block tensors: x, ctx, six modulation vectors, blk, lay, cfg, checkpoint, rows
 
 
 def _require_trainable(blk: WanBlock, cfg: WanDiTConfig) -> None:
@@ -460,22 +531,25 @@ def _require_trainable(blk: WanBlock, cfg: WanDiTConfig) -> None:
         raise ops.FvbError("the VSA backward needs the block-list sparse kernel (FVB_VSA_KERNEL=ws)")
 
 
-def _block_forward_grad(x, blk: WanBlock, ctx, temb6, lay: TokenLayout, cfg: WanDiTConfig, checkpoint: bool) -> torch.Tensor:
-    _require_trainable(blk, cfg)
-    mod = Modulation.fp32(blk, temb6)  # torch ops: autograd carries the six vectors back to scale_shift_table and temb6
+def block_forward_grad(x, blk: WanBlock, ctx, mod: Modulation, lay: TokenLayout, cfg: WanDiTConfig, checkpoint: bool) -> torch.Tensor:
+    """The block under grad (_WanBlockFn) for a modulation computed with torch ops (Modulation.fp32, or Modulation.per_frame:
+    the bf16 flow, one row per mod.rows tokens)."""
+    if mod.bf16 != (mod.rows > 0):
+        raise ops.FvbError("the block backward covers the fp32 modulation flow and the per-frame bf16 one")
     return _WanBlockFn.apply(x, ctx, mod.shift_msa, mod.scale_msa, mod.gate_msa, mod.c_shift, mod.c_scale, mod.c_gate, blk, lay,
-                             cfg, checkpoint, *(getattr(blk, n) for n in _BLOCK_TENSORS))
+                             cfg, checkpoint, mod.rows, *(getattr(blk, n) for n in _BLOCK_TENSORS))
 
 
-def checkpoint_bytes_per_block(S: int, D: int, H: int, n_tiles: int = 0) -> int:
+def checkpoint_bytes_per_block(S: int, D: int, H: int, n_tiles: int = 0, frames: int = 1) -> int:
     """Bytes a checkpointed block (block_forward(..., checkpoint=True)) keeps from its forward to its backward, for S
-    tokens of width D in H heads: the bf16 input, the fp32 modulation vectors, and the self-attention results. Dense (n_tiles
-    0): the bf16 output and the fp32 LSE. VSA (n_tiles tiles): the sparse branch's bf16 output and fp32 LSE, the block
+    tokens of width D in H heads: the bf16 input, the fp32 modulation vectors (six rows of D, or of F D for the causal model's
+    per-frame modulation over `frames` latent frames), and the self-attention results. Dense or block-causal (n_tiles 0):
+    the bf16 output and the fp32 LSE. VSA (n_tiles tiles): the sparse branch's bf16 output and fp32 LSE, the block
     means (q, k transposed with rows padded to 8 tiles; v) and the compression output, the block-score softmax (rows
     padded to 8), the int32 index lists and counts and the bool block map. The layout tables and the text states are
     shared by every block and not counted."""
     n, n8 = n_tiles, (n_tiles + 7) // 8 * 8
-    common = 2 * S * D + 6 * 4 * D + 2 * S * D + 4 * S * H
+    common = 2 * S * D + 6 * 4 * D * frames + 2 * S * D + 4 * S * H
     if not n_tiles:
         return common
     d = D // H
@@ -501,11 +575,11 @@ class _WanBlockFn(torch.autograd.Function):
     gradients are those of the forward without checkpoint."""
 
     @staticmethod
-    def forward(fctx, x, ctx, shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, blk, lay, cfg, checkpoint, *params):
+    def forward(fctx, x, ctx, shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, blk, lay, cfg, checkpoint, rows, *params):
         keep, attn = (None, {}) if checkpoint else ({}, None)
-        mod = Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate)
+        mod = Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, rows=rows, bf16=rows > 0)
         out = block_body(x.detach(), blk, ctx.detach(), mod, lay, cfg, keep, attn)
-        fctx.blk, fctx.lay, fctx.cfg, fctx.checkpoint = blk, lay, cfg, checkpoint
+        fctx.blk, fctx.lay, fctx.cfg, fctx.checkpoint, fctx.rows = blk, lay, cfg, checkpoint, rows
         if checkpoint:
             fctx.names = tuple(attn)
             fctx.save_for_backward(x, ctx, scale_msa, gate_msa, c_scale, c_gate, shift_msa, c_shift, *attn.values())
@@ -518,12 +592,12 @@ class _WanBlockFn(torch.autograd.Function):
     @staticmethod
     def backward(fctx, dout):
         x, ctx, scale_msa, gate_msa, c_scale, c_gate = fctx.saved_tensors[:6]
-        blk, lay, cfg = fctx.blk, fctx.lay, fctx.cfg
+        blk, lay, cfg, R = fctx.blk, fctx.lay, fctx.cfg, fctx.rows
         if fctx.checkpoint:
             shift_msa, c_shift, *saved = fctx.saved_tensors[6:]
             kp = {}
-            block_body(x, blk, ctx, Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate), lay, cfg, kp,
-                       dict(zip(fctx.names, saved)), replay=True)
+            block_body(x, blk, ctx, Modulation(shift_msa, scale_msa, gate_msa, c_shift, c_scale, c_gate, rows=R, bf16=R > 0), lay,
+                       cfg, kp, dict(zip(fctx.names, saved)), replay=True)
             vsa_saved = kp.pop("vsa", ())
         else:
             names = fctx.names
@@ -537,13 +611,19 @@ class _WanBlockFn(torch.autograd.Function):
         want_dctx = fctx.needs_input_grad[1]
         g = {}
         dout = dout.to(torch.bfloat16).contiguous()
+        # per-frame bf16 modulation flow (R > 0): the grouped kernels, one modulation / gate row per R tokens
+        resid_gate_bwd = ((lambda do, y_, gt, need_db: ops.resid_gate_grouped_bwd(do, y_, gt, R, need_db)) if R
+                          else ops.resid_gate_bwd)
         # feed-forward: out = bf16(x2 + o3 * c_gate), o3 = fc_out(f), f = gelu(h), h = fc_in(n3)
-        d_o3, d_cgate, g["b_2"] = ops.resid_gate_bwd(dout, kp["o3"], c_gate, need_db=need("b_2"))
+        d_o3, d_cgate, g["b_2"] = resid_gate_bwd(dout, kp["o3"], c_gate, need_db=need("b_2"))
         if need("w_2"):
             g["w_2"] = ops.linear_bwd(kp["f"], blk.w_2, d_o3, need_dx=False)[1]
         dh = ops.linear_dgrad_gelu(d_o3, blk.w_2, kp["h"])
         dn3, g["w_1"], g["b_1"] = ops.linear_bwd(kp["n3"], blk.w_1, dh, need_dw=need("w_1"), need_db=need("b_1"))
-        dx2, d_cscale, d_cshift = ops.layernorm_modulate_bwd(kp["x2"], dn3, scale=c_scale, round_ln=True, gin=dout, eps=eps)
+        if R:
+            dx2, d_cscale, d_cshift = ops.layernorm_modulate_grouped_bwd(kp["x2"], dn3, c_scale, R, gin=dout, eps=eps)
+        else:
+            dx2, d_cscale, d_cshift = ops.layernorm_modulate_bwd(kp["x2"], dn3, scale=c_scale, round_ln=True, gin=dout, eps=eps)
         # cross-attention: x2 = bf16(xb + to_out2(a2)), a2 = a2t (+ img)
         da2, g["w_o2"], g["b_o2"] = ops.linear_bwd(kp["a2"], blk.w_o2, dx2, need_dw=need("w_o2"), need_db=need("b_o2"))
         q2, kv2 = kp["q2"], kp["kv2"]
@@ -579,10 +659,11 @@ class _WanBlockFn(torch.autograd.Function):
             dctx = dctx_txt if dctx_img is None else torch.cat([dctx_img, dctx_txt], 0)
         dq2_pre, g["norm_q2"] = ops.rmsnorm_bwd(kp["q2_pre"], blk.norm_q2, dq2, eps=eps, want_dw=need("norm_q2"))
         dn2, g["w_q2"], g["b_q2"] = ops.linear_bwd(kp["n2"], blk.w_q2, dq2_pre, need_dw=need("w_q2"), need_db=need("b_q2"))
-        # norm2 of the fp32 residual y (n2 = bf16(LN(y) w + b)); xb = bf16(y) carries dx2 into dy as well
+        # norm2 of the residual y (fp32, or bf16 in the per-frame flow; n2 = bf16(LN(y) w + b)); xb = bf16(y) carries dx2 into
+        # dy as well
         dy, g["norm2_w"], g["norm2_b"] = ops.layernorm_modulate_bwd(kp["y"], dn2, weight=blk.norm2_w, gin=dx2, eps=eps)
         # self-attention out-projection: y = x + o1 * gate_msa
-        d_o1, d_gate_msa, g["b_o"] = ops.resid_gate_bwd(dy, kp["o1"], gate_msa, need_db=need("b_o"))
+        d_o1, d_gate_msa, g["b_o"] = resid_gate_bwd(dy, kp["o1"], gate_msa, need_db=need("b_o"))
         da, g["w_o"], _ = ops.linear_bwd(kp["a"], blk.w_o, d_o1, need_dw=need("w_o"))
         qkv = kp["qkv"]
         dqkv = torch.empty_like(qkv)
@@ -592,6 +673,11 @@ class _WanBlockFn(torch.autograd.Function):
             vctx.needs_input_grad = (True, True, True, True)
             dq, dk, dv, dgate = vsa._VideoSparseAttnFn.backward(vctx, hd(da))[:4]
             dqkv[:, 3 * D:].copy_(dgate.view(S, D))
+        elif lay.causal is not None:
+            c = lay.causal
+            q, k, v = hd(qkv[:, :D]), hd(qkv[:, D:2 * D]), hd(qkv[:, 2 * D:3 * D])
+            dq, dk, dv = ops.attention_sparse_bwd(q, k, v, hd(kp["a"]), kp["lse"], hd(da), c.q2k_idx, c.q2k_num, c.k2q_idx,
+                                                  c.k2q_num, q_off=c.q_off, kv_off=c.kv_off, softmax_scale=d ** -0.5)
         else:
             q, k, v = hd(qkv[:, :D]), hd(qkv[:, D:2 * D]), hd(qkv[:, 2 * D:3 * D])
             dq, dk, dv = ops.attention_bwd(q, k, v, hd(kp["a"]), kp["lse"], hd(da), softmax_scale=d ** -0.5)
@@ -599,11 +685,15 @@ class _WanBlockFn(torch.autograd.Function):
         qk_pre = kp["qk_pre"]
         g["norm_q"], g["norm_k"] = ops.rmsnorm_rope_bwd(qk_pre[:, :D], blk.norm_q, dq.reshape(S, D), dqkv[:, :D],
                                                         qk_pre[:, D:], blk.norm_k, dk.reshape(S, D), dqkv[:, D:2 * D],
-                                                        lay.cos, lay.sin, lay.rope_row, head_dim=d, eps=eps,
+                                                        lay.cos if lay.cos32 is None else lay.cos32,
+                                                        lay.sin if lay.sin32 is None else lay.sin32, lay.rope_row, head_dim=d, eps=eps,
                                                         want_dw=need("norm_q") or need("norm_k"))
         dn1, g["w_qkv"], g["b_qkv"] = ops.linear_bwd(kp["n1"], blk.w_qkv, dqkv, need_dw=need("w_qkv"), need_db=need("b_qkv"))
-        dx, d_scale_msa, d_shift_msa = ops.layernorm_modulate_bwd(x, dn1, scale=scale_msa, gin=dy, eps=eps)
-        return (dx, dctx, d_shift_msa, d_scale_msa, d_gate_msa, d_cshift, d_cscale, d_cgate, None, None, None, None,
+        if R:
+            dx, d_scale_msa, d_shift_msa = ops.layernorm_modulate_grouped_bwd(x, dn1, scale_msa, R, gin=dy, eps=eps)
+        else:
+            dx, d_scale_msa, d_shift_msa = ops.layernorm_modulate_bwd(x, dn1, scale=scale_msa, gin=dy, eps=eps)
+        return (dx, dctx, d_shift_msa, d_scale_msa, d_gate_msa, d_cshift, d_cscale, d_cgate, None, None, None, None, None,
                 *(g.get(n) if need(n) else None for n in _BLOCK_TENSORS))
 
 
@@ -674,6 +764,25 @@ class _HeadNormFn(torch.autograd.Function):
         dx, d_scale, d_shift = ops.layernorm_modulate_bwd(x, dn.to(torch.bfloat16).contiguous(), scale=scale, round_ln=True,
                                                           eps=ctx.eps)
         return dx, d_scale, d_shift, None
+
+
+class _HeadNormFramesFn(torch.autograd.Function):
+    """The causal head's norm_out with one (scale, shift) row per `rows` tokens in the bf16 modulation flow
+    (ops.layernorm_modulate with round_ln, mod_rows and mod_bf16, the no-grad call's bits); backward on
+    fvb_layernorm_modulate_grouped_bwd (dx bf16, d_scale / d_shift fp32 [F, D])."""
+
+    @staticmethod
+    def forward(ctx, x, scale, shift, rows, eps):
+        ctx.save_for_backward(x, scale)
+        ctx.rows, ctx.eps = rows, eps
+        return ops.layernorm_modulate(x, scale, shift, round_ln=True, eps=eps, mod_rows=rows, mod_bf16=True)
+
+    @staticmethod
+    def backward(ctx, dn):
+        x, scale = ctx.saved_tensors
+        dx, d_scale, d_shift = ops.layernorm_modulate_grouped_bwd(x, dn.to(torch.bfloat16).contiguous(), scale, ctx.rows,
+                                                                  eps=ctx.eps)
+        return dx, d_scale, d_shift, None, None
 
 
 # WanDiT's own trainable tensors (attribute name -> reference parameter name); the blocks' follow under blocks.{i}.

@@ -106,8 +106,9 @@ int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float* workspace,
 /* Pieces of the Wan block backward that live in GEMM epilogues (bf16 operands, the arguments of fvb_linear_bf16):
  * fvb_linear_bf16_aux: fvb_linear_bf16 that also stores the bf16 y = bf16(acc + bias) its epilogue consumes to
  *   aux[m * ldaux + n] (ldaux a multiple of 8, >= N; N a multiple of 8). Epilogues FVB_EPI_BIAS_GELU_TANH (aux = the fc_in
- *   output before the GELU), FVB_EPI_RESID_GATE_F32 and FVB_EPI_RESID_GATE_BF16 (aux = the projection before the gate
- *   multiply). `out` gets the same bits as fvb_linear_bf16, and aux the same bits as fvb_linear_bf16 with FVB_EPI_BIAS.
+ *   output before the GELU), FVB_EPI_RESID_GATE_F32, FVB_EPI_RESID_GATE_BF16 and FVB_EPI_RESID_GATE_BF16R (with its gate_rows
+ *   grouping; aux = the projection before the gate multiply). `out` gets the same bits as fvb_linear_bf16, and aux the same
+ *   bits as fvb_linear_bf16 with FVB_EPI_BIAS.
  * fvb_linear_dgrad_gelu_bf16: fvb_linear_dgrad_bf16 with the GELU(tanh) backward in its epilogue, for y = w2 . gelu(h):
  *   dh[m, k] = bf16(float(bf16(sum_n dy[m, n] * w[n, k])) * gelu_tanh'(h[m, k]))     h bf16 [M, K] (ldh a multiple of 8)
  *   gelu_tanh'(h) = 0.5 (1 + t) + 0.5 h (1 - t^2) sqrt(2/pi) (1 + 3 * 0.044715 h^2), t = tanh(sqrt(2/pi) (h + 0.044715 h^3)),
@@ -309,6 +310,38 @@ int fvb_layernorm_modulate_bwd(const void* x, int x_is_f32, int64_t ldx, const v
                                int gain_is_scale, int round_ln, const void* gin, int gin_is_f32, int64_t ldgin, void* dx,
                                int64_t lddx, float* d_gain, float* d_offset, float* workspace, int64_t workspace_bytes, int M,
                                int D, float eps, void* stream);
+
+/* Per-row-group backward of the bf16 modulation flow of the causal Wan blocks (one modulation row per latent frame).
+ * Group g is rows [g R, min((g + 1) R, M)), R = mod_rows / gate_rows > 0; its vectors are at scale + g * mod_stride (resp.
+ * gate + g * gate_stride), fp32 copies of bf16 values, stride >= the row width and a multiple of 4. G = ceil(M / R).
+ *
+ * fvb_layernorm_modulate_grouped_bwd: backward of fvb_layernorm_modulate with round_ln = 3 and mod_rows = R, whose forward is
+ *   t = bf16(LN(x)), G = bf16(1 + scale[g]), u = bf16(t G), n = bf16(u + shift[g]). x bf16 [M, D], dn bf16 [M, D]. Per row, fp32
+ *   (torch's bf16 autograd rounding points):
+ *   dt = bf16(dn * G),  dx = bf16(rstd * ((dt - mean_c(dt)) - t~ * mean_c(dt * t~)) [+ gin])   (t~ = the unrounded LN output;
+ *   gin optional, fp32 or bf16 per gin_is_f32, added before the one rounding of dx)
+ *   d_scale[g, c] = sum_{rows of g} dn * t,  d_shift[g, c] = sum_{rows of g} dn    (fp32 [G, D], row stride ld_dmod >= D)
+ *   Group sums: P = clamp(528 / G, 1, R) fixed row sets per group (rows g R + p, g R + p + P, ...) summed in row order, the P
+ *   partials added in p order; no atomics. D a multiple of 8, <= 8192; strides multiples of 8.
+ *   workspace: fvb_layernorm_modulate_grouped_bwd_workspace_bytes(M, R, D) bytes, 16-byte aligned.
+ *
+ * fvb_resid_gate_grouped_bwd: backward of FVB_EPI_RESID_GATE_BF16R, out = bf16(resid + bf16(y gate[g])), given dout bf16 [M, N]
+ *   and the saved bf16 y [M, N] (fvb_linear_bf16_aux's aux):
+ *   dy[m, n] = bf16(dout * gate[g, n])                     bf16 [M, N] (lddy)
+ *   d_gate[g, n] = sum_{rows of g} dout * y                fp32 [G, N] (row stride ld_dgate >= N)
+ *   db[n] = bf16(sum_m float(dy[m, n]))                    bf16 [N] (db NULL: skipped)
+ *   The residual's gradient is dout. Group sums as above with P = clamp(256 / G, 1, R); db adds all G P partials in (g, p)
+ *   order. N a multiple of 8; strides keep rows 16-byte aligned. workspace: fvb_resid_gate_grouped_bwd_workspace_bytes(M, R, N)
+ *   bytes, 16-byte aligned. */
+int64_t fvb_layernorm_modulate_grouped_bwd_workspace_bytes(int M, int mod_rows, int D);
+int fvb_layernorm_modulate_grouped_bwd(const void* x, int64_t ldx, const void* dn, int64_t lddn, const float* scale, int mod_rows,
+                                       int64_t mod_stride, const void* gin, int gin_is_f32, int64_t ldgin, void* dx, int64_t lddx,
+                                       float* d_scale, float* d_shift, int64_t ld_dmod, float* workspace,
+                                       int64_t workspace_bytes, int M, int D, float eps, void* stream);
+int64_t fvb_resid_gate_grouped_bwd_workspace_bytes(int M, int gate_rows, int N);
+int fvb_resid_gate_grouped_bwd(const void* dout, int64_t lddout, const void* y, int64_t ldy, const float* gate, int gate_rows,
+                               int64_t gate_stride, void* dy, int64_t lddy, float* d_gate, int64_t ld_dgate, void* db,
+                               float* workspace, int64_t workspace_bytes, int M, int N, void* stream);
 
 /* --------------------------------------------------------------------------------------------
  * Attention forward, head_dim 128, bf16, fp32 softmax. Dense or block-list (VSA / STA) keys.
