@@ -1151,6 +1151,10 @@ __global__ void __launch_bounds__(256) grouped_colsum_kernel(const float* __rest
 
 using namespace fvb;
 
+// Every pointer a row kernel reads or writes with 128-bit vectors (uint4 bf16 rows, float4 fp32 rows, per-column vectors, cos /
+// sin tables and workspace partials, double2 float64 tables) must be 16-byte aligned; NULL passes.
+static inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 extern "C" int fvb_layernorm_modulate(const void* x, int x_is_f32, int64_t ldx, const float* w, const float* b,
                                       const float* scale, const float* shift, int mod_rows, int64_t mod_stride,
                                       int round_ln, void* out, int64_t ldo, void* hidden_out, int64_t ldh, int M, int D,
@@ -1161,6 +1165,8 @@ extern "C" int fvb_layernorm_modulate(const void* x, int x_is_f32, int64_t ldx, 
   FVB_CHECK_ARG((w == nullptr) == (b == nullptr), "affine weight and bias must come together");
   FVB_CHECK_ARG((scale == nullptr) == (shift == nullptr), "scale and shift must come together");
   FVB_CHECK_ARG(mod_rows >= 0 && (mod_rows == 0 || mod_stride % 4 == 0), "bad modulation grouping (stride must be a multiple of 4)");
+  FVB_CHECK_ARG(al16(x) && al16(out) && al16(hidden_out) && al16(w) && al16(b) && al16(scale) && al16(shift),
+                "x, out, hidden_out, w, b, scale and shift must be 16-byte aligned");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   auto* o = reinterpret_cast<__nv_bfloat16*>(out);
   auto* h = reinterpret_cast<__nv_bfloat16*>(hidden_out);
@@ -1169,7 +1175,7 @@ extern "C" int fvb_layernorm_modulate(const void* x, int x_is_f32, int64_t ldx, 
   // warp-per-row kernel: 16 warps when 16 rows fit the staging budget, else as many as fit (>= 8: fp32 rows of D = 5120 are
   // 20 KB -> 9 warps x 1 stage; the block-per-row fallback ran those at 2.1 TB/s)
   const int nw = std::min(RW_WARPS, RW_SMEM_BUDGET / row_bytes);
-  const bool use_warp = M >= 256 && nw >= 8 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const bool use_warp = M >= 256 && nw >= 8;
   if (use_warp) {
     const int stages = std::max(1, std::min(RW_MAX_STAGES, RW_SMEM_BUDGET / (nw * row_bytes)));
     size_t smem = size_t(nw) * stages * row_bytes;
@@ -1214,7 +1220,8 @@ extern "C" int fvb_rmsnorm_rope_scatter(const void* x0, const void* w0, int64_t 
   FVB_CHECK_ARG(M > 0 && D > 0 && D % 128 == 0 && RW_WARPS * D * 2 <= RW_SMEM_BUDGET, "D must be a multiple of 128, <= 6144");
   FVB_CHECK_ARG(head_dim % 8 == 0 && D % head_dim == 0, "head_dim must divide D and be a multiple of 8");
   FVB_CHECK_ARG(ld0 % 8 == 0 && (x1 == nullptr || ld1 % 8 == 0) && ldy % 8 == 0, "strides must be multiples of 8");
-  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(x0) & 15) == 0 && (reinterpret_cast<uintptr_t>(x1) & 15) == 0, "rows must be 16-byte aligned");
+  FVB_CHECK_ARG(al16(x0) && al16(x1) && al16(y0) && al16(y1) && al16(w0) && al16(w1) && al16(cos_t) && al16(sin_t),
+                "x0, x1, y0, y1, w0, w1, cos and sin must be 16-byte aligned");
   FVB_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr), "cos and sin must come together");
   const int w_f32 = (rope_f64 >> 1) & 1;  // flags: bit 0 = float64 tables, bit 1 = fp32 weights
   rope_f64 &= 1;
@@ -1257,6 +1264,8 @@ extern "C" int fvb_rmsnorm_rope(void* x0, const void* w0, int64_t ld0, void* x1,
   FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
   FVB_CHECK_ARG(head_dim % 8 == 0 && D % head_dim == 0, "head_dim must divide D and be a multiple of 8");
   FVB_CHECK_ARG(ld0 % 8 == 0 && (x1 == nullptr || ld1 % 8 == 0), "strides must be multiples of 8");
+  FVB_CHECK_ARG(al16(x0) && al16(x1) && al16(w0) && al16(w1) && al16(cos_t) && al16(sin_t),
+                "x0, x1, w0, w1, cos and sin must be 16-byte aligned");
   FVB_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr), "cos and sin must come together");
   const int w_f32 = (rope_f64 >> 1) & 1;  // flags: bit 0 = float64 tables, bit 1 = fp32 weights
   rope_f64 &= 1;
@@ -1273,8 +1282,7 @@ extern "C" int fvb_rmsnorm_rope(void* x0, const void* w0, int64_t ld0, void* x1,
   FVB_CHECK_ARG(col_offsets == nullptr || D % 128 == 0, "column-block offsets need D % 128 == 0");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int row_bytes = D * 2;
-  const bool use_warp = M >= 256 && RW_WARPS * row_bytes <= RW_SMEM_BUDGET &&
-                        (reinterpret_cast<uintptr_t>(x0) & 15) == 0 && (x1 == nullptr || (reinterpret_cast<uintptr_t>(x1) & 15) == 0);
+  const bool use_warp = M >= 256 && RW_WARPS * row_bytes <= RW_SMEM_BUDGET;
   if (use_warp) {
     const int stages = rw_stages(row_bytes);
     size_t smem = size_t(RW_WARPS) * stages * row_bytes;
@@ -1307,6 +1315,7 @@ extern "C" int fvb_rmsnorm_bwd(const void* x, int64_t ldx, const void* w, const 
   FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
   FVB_CHECK_ARG(ldx % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0, "strides must be multiples of 8");
   FVB_CHECK_ARG(dw == nullptr || w != nullptr, "dw needs the weight");
+  FVB_CHECK_ARG(al16(x) && al16(w) && al16(dy) && al16(dx) && al16(workspace), "x, w, dy, dx and workspace must be 16-byte aligned");
   const int ctas = std::min(M, RB_CTAS);
   if (dw != nullptr)
     FVB_CHECK_ARG(workspace != nullptr && workspace_bytes >= fvb_rmsnorm_bwd_workspace_bytes(M, D), "workspace too small");
@@ -1332,6 +1341,7 @@ extern "C" int fvb_bias_grad_bf16(const void* dy, int64_t lddy, void* db, float*
   FVB_CHECK_ARG(dy && db && workspace, "null pointer");
   FVB_CHECK_ARG(M > 0 && N > 0 && N % 8 == 0, "N must be a positive multiple of 8");
   FVB_CHECK_ARG(lddy % 8 == 0, "lddy must be a multiple of 8");
+  FVB_CHECK_ARG(al16(dy) && al16(workspace), "dy and workspace must be 16-byte aligned");
   FVB_CHECK_ARG(workspace_bytes >= fvb_bias_grad_bf16_workspace_bytes(M, N), "workspace too small");
   const int parts = std::min(M, BG_PARTS);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1357,6 +1367,9 @@ extern "C" int fvb_rmsnorm_rope_bwd(const void* x0, int64_t ldx0, const void* w0
   FVB_CHECK_ARG(ldx0 % 8 == 0 && lddy0 % 8 == 0 && lddx0 % 8 == 0, "strides must be multiples of 8");
   FVB_CHECK_ARG(x1 == nullptr || (ldx1 % 8 == 0 && lddy1 % 8 == 0 && lddx1 % 8 == 0), "strides must be multiples of 8");
   FVB_CHECK_ARG(x1 == nullptr || (dw0 != nullptr) == (dw1 != nullptr), "dw0 and dw1 come together");
+  FVB_CHECK_ARG(al16(x0) && al16(w0) && al16(dy0) && al16(dx0) && al16(x1) && al16(w1) && al16(dy1) && al16(dx1) && al16(cos_t) &&
+                    al16(sin_t) && al16(workspace),
+                "x, w, dy, dx, cos, sin and workspace must be 16-byte aligned");
   const int ctas = std::min(M, RB_CTAS);
   const bool want_dw = dw0 != nullptr;
   if (want_dw)
@@ -1400,7 +1413,8 @@ extern "C" int fvb_resid_gate_bwd(const void* dout, int dout_is_f32, int64_t ldd
   FVB_CHECK_ARG(dout && y && gate && dy && d_gate && workspace, "null pointer");
   FVB_CHECK_ARG(M > 0 && N > 0 && N % 8 == 0, "N must be a positive multiple of 8");
   FVB_CHECK_ARG(lddout % (dout_is_f32 ? 4 : 8) == 0 && ldy % 8 == 0 && lddy % 8 == 0, "strides must keep rows 16-byte aligned");
-  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gate) & 15) == 0, "gate must be 16-byte aligned");
+  FVB_CHECK_ARG(al16(dout) && al16(y) && al16(gate) && al16(dy) && al16(workspace),
+                "dout, y, gate, dy and workspace must be 16-byte aligned");
   FVB_CHECK_ARG(workspace_bytes >= fvb_resid_gate_bwd_workspace_bytes(M, N), "workspace too small");
   const int parts = std::min(M, BG_PARTS);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -1430,7 +1444,8 @@ extern "C" int fvb_layernorm_modulate_bwd(const void* x, int x_is_f32, int64_t l
   FVB_CHECK_ARG(x && dn && gain && dx && d_gain && d_offset && workspace, "null pointer");
   FVB_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && D <= EW_THREADS * EW_MAX_CHUNKS * 8, "D must be a multiple of 8, <= 8192");
   FVB_CHECK_ARG(ldx % 8 == 0 && lddn % 8 == 0 && lddx % 8 == 0 && (gin == nullptr || ldgin % 8 == 0), "strides must be multiples of 8");
-  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gain) & 15) == 0, "gain must be 16-byte aligned");
+  FVB_CHECK_ARG(al16(x) && al16(dn) && al16(gain) && al16(gin) && al16(dx) && al16(workspace),
+                "x, dn, gain, gin, dx and workspace must be 16-byte aligned");
   FVB_CHECK_ARG(workspace_bytes >= fvb_layernorm_modulate_bwd_workspace_bytes(M, D), "workspace too small");
   FVB_CHECK_ARG(gain_is_scale || !round_ln, "round_ln belongs to the modulation form (the affine forward rounds after w, b)");
   const int ctas = std::min(M, RB_CTAS);
@@ -1465,7 +1480,8 @@ extern "C" int fvb_layernorm_modulate_grouped_bwd(const void* x, int64_t ldx, co
   FVB_CHECK_ARG(mod_rows > 0 && mod_stride % 4 == 0 && mod_stride >= D, "bad modulation grouping (rows > 0, stride >= D and a multiple of 4)");
   FVB_CHECK_ARG(ldx % 8 == 0 && lddn % 8 == 0 && lddx % 8 == 0 && (gin == nullptr || ldgin % 8 == 0), "strides must be multiples of 8");
   FVB_CHECK_ARG(ld_dmod >= D, "ld_dmod must be >= D");
-  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(scale) & 15) == 0, "scale must be 16-byte aligned");
+  FVB_CHECK_ARG(al16(x) && al16(dn) && al16(scale) && al16(gin) && al16(dx) && al16(workspace),
+                "x, dn, scale, gin, dx and workspace must be 16-byte aligned");
   FVB_CHECK_ARG(workspace_bytes >= fvb_layernorm_modulate_grouped_bwd_workspace_bytes(M, mod_rows, D), "workspace too small");
   const int G = (M + mod_rows - 1) / mod_rows;
   const int parts = grouped_parts(M, mod_rows, RB_CTAS);
@@ -1504,7 +1520,8 @@ extern "C" int fvb_resid_gate_grouped_bwd(const void* dout, int64_t lddout, cons
   FVB_CHECK_ARG(gate_rows > 0 && gate_stride % 4 == 0 && gate_stride >= N, "bad gate grouping (rows > 0, stride >= N and a multiple of 4)");
   FVB_CHECK_ARG(lddout % 8 == 0 && ldy % 8 == 0 && lddy % 8 == 0, "strides must keep rows 16-byte aligned");
   FVB_CHECK_ARG(ld_dgate >= N, "ld_dgate must be >= N");
-  FVB_CHECK_ARG((reinterpret_cast<uintptr_t>(gate) & 15) == 0, "gate must be 16-byte aligned");
+  FVB_CHECK_ARG(al16(dout) && al16(y) && al16(gate) && al16(dy) && al16(workspace),
+                "dout, y, gate, dy and workspace must be 16-byte aligned");
   FVB_CHECK_ARG(workspace_bytes >= fvb_resid_gate_grouped_bwd_workspace_bytes(M, gate_rows, N), "workspace too small");
   const int G = (M + gate_rows - 1) / gate_rows;
   const int parts = grouped_parts(M, gate_rows, BG_PARTS);

@@ -219,6 +219,15 @@ int fvb_gemm_batched_bf16(const void* a, int64_t lda, int64_t a_batch_stride, co
                           int batch, float div, void* stream);
 
 /* --------------------------------------------------------------------------------------------
+ * Row kernels: fvb_layernorm_modulate, fvb_rmsnorm_rope, fvb_rmsnorm_rope_scatter and the backward entry points below
+ * (fvb_rmsnorm_bwd, fvb_rmsnorm_rope_bwd, fvb_layernorm_modulate_bwd, the two grouped ones), plus fvb_bias_grad_bf16 and
+ * fvb_resid_gate_bwd above. They access their rows, per-column vectors (w, b, scale, shift, gain, gate), cos / sin tables
+ * and workspace with 128-bit vectors: every such pointer must be 16-byte aligned, else the call returns
+ * FVB_ERR_INVALID_ARG. Outputs written one element at a time (dw, db, d_gate, d_gain, d_offset, d_scale, d_shift) and
+ * index arrays (rope_row, col_offsets) need only their natural alignment.
+ * -------------------------------------------------------------------------------------------- */
+
+/* --------------------------------------------------------------------------------------------
  * LayerNorm + AdaLN modulation (one pass over the row, fp32 statistics)
  * Replaces: FP32LayerNorm / ScaleResidualLayerNormScaleShift / LayerNormScaleShift
  *   (fastvideo/layers/layernorm.py:115-125, 159-213, 216-273) as used at

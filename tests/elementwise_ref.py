@@ -63,6 +63,31 @@ error 2^-22 (ex2.approx.f32 in the wgmma kernels; exp2f, at most 2 fp32 ulp, in 
 delta's fp32 sum (128 U32 sum |dO o|), the roundings of P (dP - delta) scale, the bf16 rounding of P and dS (half an ulp
 each), the second GEMM's chain (acc_coeff(rows walked) sum |bf16(.)| |operand|) and the final bf16 store, element by
 element as [B, H, Sq, Skv] fp64 tensors followed by a matmul with |operand|.
+
+Row kernels (csrc/elementwise.cu: LayerNorm-modulation, RMSNorm + RoPE, their backwards, the bias and gated-residual
+column sums), three tiers:
+(a) Exact forward rows (exact_rows): x = c + z, c and z on the grid a * 2^-4, z the pairs +-a permuted so sum z = 0 exactly.
+    The row sum D c, sum (x - mean)^2 = sum z^2 and sum x^2 are integer numbers of 2^-8 quanta below 2^24: exact in fp32 in
+    any order, with or without fma. The only steps left that are not IEEE are the statistics' forms and rsqrtf:
+    mean_forms gives s / D (block-per-row) and s fl(1/D) (warp-per-row), and exact_rows asserts that both equal c (a row
+    where they would not gets c = 0). var_forms gives fl(fl(q / D) + eps), fl(fl(q fl(1/D)) + eps) and the fused
+    fl(q fl(1/D) + eps). rstd_candidates collects every fp32 value within 2 ulp (rsqrtf's documented maximum error) of
+    1 / sqrt(v) for each form. assert_rows_match then requires each output row to equal, bit for bit, the documented
+    rounding chain (ln_chain, rms_rope_chain: separate torch fp32 / float64 ops) at one candidate rstd, the same one for
+    the whole row. With D a power of two both paths compute the same statistics, so they must give identical bits.
+(b) Exact column sums: every summed term (dn bf16(t), dy bf16(x^), dout y, dn, dy) is a product of bf16 values or a bf16
+    value, exact in fp32, so the kernels' fma is a plain add and colsum_replay / grouped_colsum_replay replay the
+    documented order bit for bit: part p adds rows p, p + P, ... in row order, the partials are added in part order
+    (grouped: P = clamp(budget / G, 1, R) per group, db over all G P partials in (g, p) order). Where the rstd candidates
+    disagree on bf16(t) or bf16(x^) for an element (unambiguous_bf16), the test sets that element's dn / dy to 0.
+(c) fp64 element bounds on random rows. _stats64: the mean carries gamma(D) of sum |x| plus the division's rounding; the
+    variance gamma(D + 2) relative plus the mean error squared (sum (x - m')^2 = sum d^2 + D (m - m')^2); rstd half of
+    that plus rsqrtf's 2^-22 and one rounding (rho). ln_fwd_bound carries t's error (rho |t| + rstd e_mean) through every
+    fp32 rounding (u of the magnitude) and bf16 rounding (half an ulp) of the chain, each multiplied by the factor of the
+    later steps (|w|, |1 + scale|, |cos|, |sin|). norm_bwd_dx_bound does the same for dx: the two row sums (gamma(D) of
+    their magnitude sums), rstd, t or x^, and the roundings of the formula of include/fvb200.h; dt itself (bf16(dy w), the
+    un-rotated dn, dn gain) is replayed exactly. The largest error / bound ratios sit near 1: the final bf16 rounding is
+    half an ulp, and the bounds add little else.
 """
 import math
 
@@ -291,13 +316,15 @@ class Guarded:
     """A buffer of random bytes; a kernel writes into views of it (view()), and assert_untouched() checks that every
     element outside the registered regions still holds its original bits."""
 
-    def __init__(self, shape, dtype, device, seed=0):
+    def __init__(self, shape, dtype, device, seed=0, fill=None):
         self.buf = torch.empty(tuple(shape), dtype=dtype, device=device)
         g = torch.Generator(device=device).manual_seed(seed)
         raw = torch.randint(-2 ** 15, 2 ** 15, (self.buf.numel() * self.buf.element_size() // 2,), generator=g,
                             device=device, dtype=torch.int32).to(torch.int16)
         self.buf.view(-1).view(torch.int16).copy_(raw)
-        if dtype.is_floating_point:  # keep the pattern finite, so views that a kernel also reads stay usable
+        if fill is not None:  # e.g. NaN: a workspace whose every partial must be written before it is read
+            self.buf.fill_(fill)
+        elif dtype.is_floating_point:  # keep the pattern finite, so views that a kernel also reads stay usable
             iv = self.buf.view(_INT_VIEW[dtype])
             bad = ~torch.isfinite(self.buf)
             iv[bad] = iv[bad] & ~(1 << (14 if dtype == torch.bfloat16 else 30))
@@ -629,3 +656,298 @@ def bwd_coords(idx):
     """Element (b, row, h, col) of dq / dk / dv -> the CTA (128 owned rows), consumer warpgroup and 8-column group."""
     b, r, h, c = (int(i) for i in idx)
     return dict(b=b, row=r, h=h, col=c, cta=r // 128, warpgroup=(r % 128) // 64, col_group=c // 8)
+
+
+# ------------------------------------------------------------------------------------------------ row kernels
+# The HBM-bound row kernels of csrc/elementwise.cu (module docstring: "Row kernels").
+RB_CTAS, BG_PARTS = 528, 256  # the fixed row-set counts of the backward column sums
+
+
+def _step_ulps(r, k):
+    """fp32 r moved k ulps (k < 0: down)."""
+    toward = torch.full_like(r, math.inf if k > 0 else -math.inf)
+    for _ in range(abs(k)):
+        r = torch.nextafter(r, toward)
+    return r
+
+
+def mean_forms(s, D):
+    """The fp32 means the kernels may compute from the fp32 row sum s: s / D (block-per-row, IEEE division) and
+    s * fl(1 / D) (warp-per-row)."""
+    Dt = torch.full_like(s, float(D))
+    return [s / Dt, s * (torch.ones_like(s) / Dt)]
+
+
+def var_forms(q, D, eps, warp):
+    """fp32 values of q / D + eps the kernels may compute from the exact fp32 sum q: fl(fl(q / D) + eps) in the
+    block-per-row kernels; fl(fl(q fl(1 / D)) + eps) or, contracted to one fma, fl(q fl(1 / D) + eps) in the warp-per-row
+    ones (q fl(1/D) is exact in fp64, and so is its sum with eps at these magnitudes)."""
+    Dt = torch.full_like(q, float(D))
+    e = torch.full_like(q, f32(eps))
+    out = [q / Dt + e]
+    if warp:
+        inv = torch.ones_like(q) / Dt
+        out += [q * inv + e, (q.double() * inv.double() + e.double()).float()]
+    return out
+
+
+def rstd_candidates(vs):
+    """fp32 [M, K]: for each form v of the variance (var_forms), every fp32 value within 2 ulp of 1 / sqrt(v) (rsqrtf's
+    documented maximum error); entries outside that range repeat the rounded value."""
+    cands = []
+    for v in vs:
+        r64 = 1.0 / v.double().sqrt()
+        base = r64.float()
+        for k in range(-2, 3):
+            c = _step_ulps(base, k)
+            cands.append(torch.where((c.double() - r64).abs() <= 2 * ulp_f32(r64), c, base))
+    return torch.stack(cands, 1)
+
+
+def exact_rows(M, D, gen, device, lim=15):
+    """Rows x = c + z, fp32 [M, D] values that bf16 holds exactly (module docstring (a)): z is the pairs +-a * 2^-4
+    (1 <= a <= lim) in a random order per row, so sum z = 0 exactly; c = a * 2^-4 (|a| <= lim), or 0 for a row where a mean
+    form of D c would not give c back. Then every sum the kernels form (sum x = D c, sum (x - mean)^2 = sum z^2,
+    sum x^2 = D c^2 + sum z^2) is an integer number of 2^-8 quanta below 2^24, exact in fp32 in any order. Returns x, c [M]
+    and the exact fp32 sums sum z^2 and sum x^2."""
+    assert D % 2 == 0
+    a = torch.randint(1, lim + 1, (M, D // 2), generator=gen, device=device).float()
+    z = torch.cat([a, -a], 1).gather(1, torch.rand(M, D, generator=gen, device=device).argsort(1)) * 2.0 ** -4
+    c = torch.randint(-lim, lim + 1, (M,), generator=gen, device=device).float() * 2.0 ** -4
+    ok = torch.ones(M, dtype=torch.bool, device=device)
+    for m in mean_forms(c * D, D):
+        ok &= m == c
+    c = torch.where(ok, c, torch.zeros_like(c))
+    x = c[:, None] + z
+    assert bool((x.bfloat16().float() == x).all())
+    for m in mean_forms(x.double().sum(1).float(), D):  # the premise: every mean form is c
+        assert bool((m == c).all()), "exact rows: a mean form differs from c"
+    qz, qx = (z.double() ** 2).sum(1), (x.double() ** 2).sum(1)
+    assert bool((qx * 256 < 2 ** 24).all()), "exact rows: sum x^2 reaches 2^24 quanta"
+    return x, c, qz.float(), qx.float()
+
+
+def ln_chain(x, mean, rstd, w=None, b=None, scale=None, shift=None, round_ln=0):
+    """fvb_layernorm_modulate's output for fp32 mean / rstd [M], rounding for rounding with torch fp32 ops (include/fvb200.h):
+    t = (x - mean) rstd [* w + b], bf16(t) with round_ln & 1, the fp32 modulation t (1 + scale) + shift or, with round_ln & 2,
+    bf16(bf16(t bf16(1 + scale)) + shift). scale / shift: fp32 [D] or already expanded to [M, D]."""
+    t = (x.float() - mean[:, None]) * rstd[:, None]
+    if w is not None:
+        t = t * w + b
+    if round_ln & 1:
+        t = t.bfloat16().float()
+    if scale is not None:
+        gain = torch.ones_like(scale) + scale
+        if round_ln & 2:
+            t = ((t * gain.bfloat16().float()).bfloat16().float() + shift).bfloat16().float()
+        else:
+            t = t * gain + shift
+    return t.bfloat16()
+
+
+def rope_chain(n, cos, sin, f64=False):
+    """The interleaved-pair rotation of fvb_rmsnorm_rope on fp32 n [M, D] with per-element table values cos / sin [M, D]
+    (fp32, or float64 with f64): fp32 o0 = fl(fl(n0 c0) + fl(-n1 s0)), o1 = fl(fl(n1 c1) + fl(n0 s1)); float64: the same in
+    float64, then double -> float. Returns fp32 (rounded to bf16 by the caller)."""
+    n0, n1 = n[:, 0::2], n[:, 1::2]
+    c0, c1, s0, s1 = cos[:, 0::2], cos[:, 1::2], sin[:, 0::2], sin[:, 1::2]
+    if f64:
+        n0, n1 = n0.double(), n1.double()
+        y0, y1 = (n0 * c0 + (-n1) * s0).float(), (n1 * c1 + n0 * s1).float()
+    else:
+        y0, y1 = n0 * c0 + (-n1) * s0, n1 * c1 + n0 * s1
+    return torch.stack([y0, y1], -1).flatten(1)
+
+
+def rms_rope_chain(x, rstd, w=None, w_f32=False, cos=None, sin=None, f64=False):
+    """fvb_rmsnorm_rope's output for fp32 rstd [M]: n = bf16(bf16(x rstd) w) (bf16 w), bf16(x rstd) w unrounded (fp32 w),
+    n = x without w (the scatter's RoPE-only mode); then the rotation when tables are given, and one bf16 rounding."""
+    n = x.float()
+    if w is not None:
+        n = (n * rstd[:, None]).bfloat16().float() * w.float()
+        if not w_f32:
+            n = n.bfloat16().float()
+    if cos is not None:
+        n = rope_chain(n, cos, sin, f64)
+    return n.bfloat16()
+
+
+def row_coords(row, col, nw=None, grid=None):
+    """A failing element -> its row, column, 8-column chunk, lane (chunk % 32 of the warp path) and, given the warp
+    path's nw and grid, the CTA, warp and ring iteration that own the row."""
+    d = dict(row=row, col=col, chunk=col // 8, lane=(col // 8) % 32)
+    if nw:
+        d.update(cta=(row // nw) % grid, warp=row % nw, iteration=row // (nw * grid))
+    return d
+
+
+def assert_rows_match(got, chain, cands, name, where=None, family=None):
+    """Each row of got (bf16 [M, D]) equals chain(rstd) bit for bit for one candidate rstd of that row (cands [M, K]), the
+    same candidate for every element of the row. Returns the index of the matching candidate per row."""
+    M = got.shape[0]
+    hit = torch.full((M,), -1, dtype=torch.int64, device=got.device)
+    for k in range(cands.shape[1]):
+        ok = (chain(cands[:, k]) == got).all(-1) & (hit < 0)
+        hit[ok] = k
+    bad = hit < 0
+    if bool(bad.any()):
+        rows = bad.nonzero().flatten()
+        r = int(rows[0])
+        ref = chain(cands[:, 0])[r]
+        cols = (ref != got[r]).nonzero().flatten()[:8].tolist()
+        desc = [where(r, c) if where else dict(row=r, col=c) for c in cols]
+        raise AssertionError(f"{name}: {rows.numel()} rows match no candidate rstd; first {desc}")
+    if family:
+        note_exact(family, got.numel())
+    return hit
+
+
+def unambiguous_bf16(vals):
+    """vals [K, ...] (fp32 candidates of one quantity) -> (bf16(vals[0]) as fp32, mask where every candidate rounds to the
+    same bf16)."""
+    b = vals.bfloat16().float()
+    return b[0], (b == b[0]).all(0)
+
+
+def colsum_replay(T, parts):
+    """Column sums of fp32 terms T [M, N] in the kernels' order: part p adds rows p, p + parts, ... in row order (one fp32
+    rounding per add, the fma of an exact product being a plain add), then the partials are added in part order. Returns
+    (sum fp32 [N], partials fp32 [parts, N])."""
+    M, N = T.shape
+    steps = -(-M // parts)
+    Tp = torch.cat([T.float(), T.new_zeros(steps * parts - M, N)]).view(steps, parts, N)
+    acc = T.new_zeros(parts, N)
+    for s in range(steps):
+        acc = acc + Tp[s]
+    return partial_sum(acc), acc
+
+
+def partial_sum(acc):
+    """acc [P, N] added in row order with fp32 adds."""
+    tot = acc.new_zeros(acc.shape[1:])
+    for p in range(acc.shape[0]):
+        tot = tot + acc[p]
+    return tot
+
+
+def grouped_parts(M, R, budget):
+    """P of the grouped backwards: clamp(budget / G, 1, R), G = ceil(M / R)."""
+    G = -(-M // R)
+    return max(1, min(R, budget // G))
+
+
+def grouped_colsum_replay(T, R, budget):
+    """Group sums of the grouped backwards: group g = rows [g R, min((g + 1) R, M)), P = grouped_parts(M, R, budget) row
+    sets per group (rows g R + p, g R + p + P, ...) in row order, the group's partials added in p order; a part with no rows
+    contributes an all-zero partial. Returns (sums fp32 [G, N], partials fp32 [G, P, N] in (g, p) order)."""
+    M, N = T.shape
+    G, P = -(-M // R), grouped_parts(M, R, budget)
+    steps = -(-R // P)
+    Tp = torch.cat([T.float(), T.new_zeros(G * R - M, N)]).view(G, R, N)
+    Tp = torch.cat([Tp, T.new_zeros(G, steps * P - R, N)], 1).view(G, steps, P, N)
+    acc = T.new_zeros(G, P, N)
+    for s in range(steps):
+        acc = acc + Tp[:, s]
+    tot = T.new_zeros(G, N)
+    for p in range(P):
+        tot = tot + acc[:, p]
+    return tot, acc
+
+
+def gamma(n):
+    """Bound on the relative error of an n-term fp32 sum in any order (n u / (1 - n u))."""
+    return n * U32 / (1 - n * U32)
+
+
+def _stats64(x, D, eps, centred):
+    """fp64 mean, rstd and the kernel's rstd relative error bound rho (module docstring (c))."""
+    x = x.double()
+    mean = x.mean(1) if centred else torch.zeros_like(x[:, 0])
+    d = x - mean[:, None]
+    var = (d * d).mean(1)
+    e_mean = (gamma(D) * x.abs().sum(1) / D + U32 * mean.abs()) if centred else torch.zeros_like(mean)
+    # sum (x - m')^2 = sum d^2 + D (m - m')^2; the fp32 sum, the division and the + eps add one rounding each
+    rel_v = (gamma(D + 2) * var + e_mean ** 2) / (var + eps)
+    rho = 0.5 * rel_v / (1 - rel_v) + 2.0 ** -22 + U32
+    return mean, 1.0 / (var + f32(eps)).sqrt(), rho, e_mean
+
+
+def ln_fwd_bound(x, eps, w=None, b=None, scale=None, shift=None, round_ln=0, rms=False, rms_w=None, rms_w_f32=False,
+                 cos=None, sin=None):
+    """fp64 reference and element bound of fvb_layernorm_modulate (rms=False) or fvb_rmsnorm_rope (rms=True) on random rows.
+    Per element: t's error from rstd (rho |t|) and the mean (rstd e_mean), then every fp32 rounding (u of the magnitude) and
+    bf16 rounding (half an ulp) of the chain, each carried through the later steps with its factor."""
+    M, D = x.shape
+    mean, r, rho, e_mean = _stats64(x, D, eps, not rms)
+    d = x.double() - mean[:, None]
+    t = d * r[:, None]
+    et = t.abs() * rho[:, None] + r[:, None] * e_mean[:, None] + U32 * (t.abs() + r[:, None] * e_mean[:, None])
+    if rms:
+        et = et + half_ulp_bf16(t.abs() + et)  # bf16(x rstd)
+        if rms_w is not None:
+            wv = rms_w.double()
+            t, et = t * wv, et * wv.abs() + U32 * (t * wv).abs()
+            if not rms_w_f32:
+                et = et + half_ulp_bf16(t.abs() + et)
+        if cos is not None:
+            c, s = cos.double(), sin.double()
+            t0, t1, e0, e1 = t[:, 0::2], t[:, 1::2], et[:, 0::2], et[:, 1::2]
+            c0, c1, s0, s1 = c[:, 0::2], c[:, 1::2], s[:, 0::2], s[:, 1::2]
+            y0, y1 = t0 * c0 - t1 * s0, t1 * c1 + t0 * s1
+            b0 = e0 * c0.abs() + e1 * s0.abs() + 2 * U32 * ((t0 * c0).abs() + (t1 * s0).abs() + y0.abs())
+            b1 = e1 * c1.abs() + e0 * s1.abs() + 2 * U32 * ((t1 * c1).abs() + (t0 * s1).abs() + y1.abs())
+            t, et = torch.stack([y0, y1], -1).flatten(1), torch.stack([b0, b1], -1).flatten(1)
+        return t, et + half_ulp_bf16(t.abs() + et)
+    if w is not None:
+        wv, bv = w.double(), b.double()
+        tw = t * wv
+        t, et = tw + bv, et * wv.abs() + U32 * (tw.abs() + (tw + bv).abs())
+    if round_ln & 1:
+        et = et + half_ulp_bf16(t.abs() + et)
+    if scale is not None:
+        g = 1.0 + scale.double()
+        ge = U32 * g.abs()
+        if round_ln & 2:
+            ge = half_ulp_bf16(g.abs() + ge)
+        tg = t * g
+        etg = et * g.abs() + t.abs() * ge
+        etg = etg + (half_ulp_bf16(tg.abs() + etg) if round_ln & 2 else U32 * tg.abs())
+        t = tg + shift.double()
+        et = etg + (half_ulp_bf16(t.abs() + etg) if round_ln & 2 else U32 * t.abs())
+    return t, et + half_ulp_bf16(t.abs() + et)
+
+
+def norm_bwd_dx_bound(x, dt, eps, rms, gin=None):
+    """fp64 reference and element bound of dx for the RMSNorm (rms) and LayerNorm backwards, given the kernel's exact fp32
+    dt per element (bf16(dy w), the un-rotated dn, dn * gain or bf16(dn bf16(1 + scale)): replayed, not bounded).
+    RMSNorm: dx = r (g - x^ (r s / D)), s = sum g x; LayerNorm: dx = rstd ((dt - mean(dt)) - t mean(dt t)). The sums' errors
+    (gamma(D) of their magnitude sums), rstd's (rho), t's and every fp32 rounding are carried element by element; the
+    result is then rounded once (fp32 dx: u; bf16 dx: half a bf16 ulp, added by the caller's choice of `bf16`)."""
+    M, D = x.shape
+    mean, r, rho, e_mean = _stats64(x, D, eps, not rms)
+    r2 = r[:, None]
+    dt = dt.double()
+    d = x.double() - mean[:, None]
+    xh = d * r2
+    exh = xh.abs() * rho[:, None] + r2 * e_mean[:, None] + U32 * (xh.abs() + r2 * e_mean[:, None])
+    if rms:
+        s = (dt * x.double()).sum(1, keepdim=True)
+        es = gamma(D) * (dt * x.double()).abs().sum(1, keepdim=True)
+        k = r2 * s / D
+        ek = (es * r2 + s.abs() * r2 * rho[:, None]) / D + 2 * U32 * k.abs()
+        a = dt - xh * k
+        ea = exh * k.abs() + xh.abs() * ek + U32 * ((xh * k).abs() + a.abs())
+    else:
+        mdt = dt.mean(1, keepdim=True)
+        emdt = gamma(D) * dt.abs().mean(1, keepdim=True) + U32 * mdt.abs()
+        mdx = (dt * xh).mean(1, keepdim=True)
+        emdx = gamma(D) * (dt * xh).abs().mean(1, keepdim=True) + (dt.abs() * exh).mean(1, keepdim=True) + U32 * mdx.abs()
+        a1 = dt - mdt
+        a = a1 - xh * mdx
+        ea = emdt + U32 * a1.abs() + exh * mdx.abs() + xh.abs() * emdx + U32 * ((xh * mdx).abs() + a.abs())
+    o = r2 * a
+    eo = r2 * ea + o.abs() * rho[:, None] + U32 * o.abs()
+    if gin is not None:
+        o = o + gin.double()
+        eo = eo + U32 * o.abs()
+    return o, eo

@@ -395,3 +395,215 @@ def test_attention_bwd_checkers_reject_defects(kind):
         mq, mk, mv, _ = sim(l=l2)
         rejects(mq, dk, dv)
         rejects(dq, dk, mv)
+
+
+# ------------------------------------------------------------------------------------------------ row kernels
+def _sim_rstd(x, D, eps, warp, centred, mean=None):
+    """The kernels' statistics in torch fp32: block-per-row sums (256 per-thread partials, then a tree) with IEEE division,
+    or warp-per-row pairwise sums over the 32 lanes with a multiply by fl(1 / D) fused into one fma; rsqrt rounded to
+    fp32 and moved one ulp (within rsqrtf's 2 ulp)."""
+    xf = x.float()
+    M = xf.shape[0]
+    lanes = 32 if warp else 256
+    pad = (-D) % (8 * lanes)
+    xp = torch.cat([xf, xf.new_zeros(M, pad)], 1).view(M, -1, lanes, 8)
+
+    def tree(v):  # per-lane sums in chunk order, then a butterfly over the lanes
+        acc = v[:, 0].sum(-1)
+        for k in range(1, v.shape[1]):
+            acc = acc + v[:, k].sum(-1)
+        while acc.shape[1] > 1:
+            acc = acc[:, 0::2] + acc[:, 1::2]
+        return acc[:, 0]
+
+    Dt = torch.full((M,), float(D))
+    inv = torch.ones(M) / Dt
+    if centred:
+        s = tree(xp)
+        mean = s * inv if warp else s / Dt
+        d = xp - torch.where(torch.arange(xp.shape[1] * lanes * 8).view(1, -1, lanes, 8) < D, mean[:, None, None, None], xp)
+        q = tree(d * d)
+    else:
+        mean = torch.zeros(M)
+        q = tree(xp * xp)
+    v = (q.double() * inv.double() + R.f32(eps)).float() if warp else q / Dt + torch.full((M,), R.f32(eps))
+    r = torch.nextafter((1.0 / v.double().sqrt()).float(), torch.full((M,), math.inf))
+    return mean, r
+
+
+def _row_sim(M, D, seed, f32_rows=False):
+    g = _gen(seed)
+    x, c, qz, qx = R.exact_rows(M, D, g, CPU)
+    return (x if f32_rows else x.bfloat16()), c, qz, qx, g
+
+
+@pytest.mark.parametrize("warp", [False, True])
+@pytest.mark.parametrize("D", [8, 264, 1536, 2056, 5120])
+def test_layernorm_reference_accepts_the_kernel_arithmetic(D, warp):
+    """Exact rows: the simulated kernel (either path's sum order, a perturbed rsqrt) equals ln_chain at one candidate rstd
+    per row, for every modulation form; the fp64 bound accepts the simulation on random rows."""
+    x, c, qz, _, g = _row_sim(40, D, D)
+    mean, r = _sim_rstd(x, D, 1e-6, warp, True)
+    assert torch.equal(mean, c)
+    cands = R.rstd_candidates(R.var_forms(qz, D, 1e-6, warp))
+    w, b, sc, sh = (torch.randn(D, generator=g) * 0.5 for _ in range(4))
+    for kw in (dict(round_ln=1, scale=sc, shift=sh), dict(w=w, b=b), dict(round_ln=3, scale=sc.bfloat16().float(),
+                                                                            shift=sh.bfloat16().float())):
+        got = R.ln_chain(x, mean, r, **kw)
+        R.assert_rows_match(got, lambda rr: R.ln_chain(x, c, rr, **kw), cands, "sim")
+        xr = (torch.randn(40, D, generator=g) * 2 + 1).bfloat16()
+        m2, r2 = _sim_rstd(xr, D, 1e-6, warp, True)
+        ref, bound = R.ln_fwd_bound(xr.float(), 1e-6, **kw)
+        R.assert_within(R.ln_chain(xr, m2, r2, **kw), ref, bound, "sim random")
+
+
+def test_layernorm_checkers_reject_wrong_statistics_and_groups():
+    """One row normalised with the previous row's statistics, and the last rows of a modulation group given the next
+    group's vectors: both fail the exact check (and the statistics defect the bound)."""
+    M, D, Rg = 24, 1536, 10
+    x, c, qz, _, g = _row_sim(M, D, 1)
+    cands = R.rstd_candidates(R.var_forms(qz, D, 1e-6, True))
+    mean, r = _sim_rstd(x, D, 1e-6, True, True)
+    sc, sh = torch.randn(3, D, generator=g), torch.randn(3, D, generator=g)
+    grp = torch.arange(M) // Rg
+    chain = lambda rr: R.ln_chain(x, c, rr, scale=sc[grp], shift=sh[grp], round_ln=1)
+    m2, r2 = mean.clone(), r.clone()
+    m2[7], r2[7] = mean[6], r[6]
+    with pytest.raises(AssertionError, match="match no candidate"):
+        R.assert_rows_match(R.ln_chain(x, m2, r2, scale=sc[grp], shift=sh[grp], round_ln=1), chain, cands, "stats")
+    grp2 = grp.clone()
+    grp2[8:10] = 1
+    with pytest.raises(AssertionError, match="match no candidate"):
+        R.assert_rows_match(R.ln_chain(x, mean, r, scale=sc[grp2], shift=sh[grp2], round_ln=1), chain, cands, "group")
+    xr = (torch.randn(M, D, generator=g) * 2 + torch.randn(M, 1, generator=g)).bfloat16()
+    m3, r3 = _sim_rstd(xr, D, 1e-6, True, True)
+    ref, bound = R.ln_fwd_bound(xr.float(), 1e-6)
+    m3[7], r3[7] = m3[6], r3[6]
+    with pytest.raises(AssertionError, match="outside the element bound"):
+        R.assert_within(R.ln_chain(xr, m3, r3), ref, bound, "stats random")
+
+
+def _rope_case(M, D, hd, f64, g):
+    x, c, qz, qx = R.exact_rows(M, D, g, CPU)
+    x = x.bfloat16()
+    S = M + 5
+    prow = torch.randperm(S, generator=g)[:M]
+    ang = torch.rand(S, hd // 2, generator=g, dtype=torch.float64) * 6.3
+    cos, sin = (f(ang).repeat_interleave(2, 1) for f in (torch.cos, torch.sin))
+    if not f64:
+        cos, sin = cos.float(), sin.float()
+    cols = torch.arange(D) % hd
+    w = (torch.randn(D, generator=g) * 0.5 + 1).bfloat16()
+    return x, qx, w, prow, cos, sin, cols
+
+
+@pytest.mark.parametrize("f64", [False, True])
+@pytest.mark.parametrize("hd", [24, 128, 512])
+def test_rmsnorm_rope_reference_accepts_and_rejects(hd, f64):
+    """The simulated kernel matches rms_rope_chain at one candidate per row; a table slice 8 columns off inside a head,
+    cos and sin swapped, and rope_row ignored all fail."""
+    M, D = 16, 1536
+    x, qx, w, prow, cos, sin, cols = _rope_case(M, D, hd, f64, _gen(hd))
+    _, r = _sim_rstd(x, D, 1e-6, True, False)
+    cands = R.rstd_candidates(R.var_forms(qx, D, 1e-6, True))
+    ce, se = cos[prow][:, cols], sin[prow][:, cols]
+    chain = lambda rr: R.rms_rope_chain(x, rr, w, False, ce, se, f64)
+    R.assert_rows_match(R.rms_rope_chain(x, r, w, False, ce, se, f64), chain, cands, "sim")
+    shifted = (cols // hd) * hd + (cols % hd + 8) % hd
+    for name, (c2, s2) in {"shift 8": (cos[prow][:, shifted], sin[prow][:, shifted]), "swap": (se, ce),
+                           "rope_row ignored": (cos[:M][:, cols], sin[:M][:, cols])}.items():
+        with pytest.raises(AssertionError, match="match no candidate"):
+            R.assert_rows_match(R.rms_rope_chain(x, r, w, False, c2, s2, f64), chain, cands, name)
+
+
+def _sim_colsum(T, parts, order=None, drop=None, twice=None):
+    """Kernel-style column sums with optional defects: partials added in another order, one dropped or added twice."""
+    _, acc = R.colsum_replay(T, parts)
+    idx = list(range(parts)) if order is None else order
+    if drop is not None:
+        idx.remove(drop)
+    if twice is not None:
+        idx.append(twice)
+    return R.partial_sum(acc[idx])
+
+
+@pytest.mark.parametrize("M,N", [(2048, 1032), (1793, 8), (529, 1536)])
+def test_column_sum_replay_and_its_defects(M, N):
+    """The replay equals a row-by-row fp32 simulation of the kernels (including the 8-row unrolled loop, which keeps
+    the order); a dropped, doubled or reordered partial and a missing last 1024-column block all change the bits."""
+    g = _gen(M + N)
+    T = R.rand_bf16((M, N), g, CPU).float()
+    parts = min(M, R.BG_PARTS if M != 529 else R.RB_CTAS)
+    acc = torch.zeros(parts, N)
+    for row in range(M):  # the kernel's loop, one row at a time
+        acc[row % parts] = acc[row % parts] + T[row]
+    ref = R.colsum_replay(T, parts)[0]
+    assert torch.equal(R.partial_sum(acc), ref)
+    defects = {"dropped": _sim_colsum(T, parts, drop=parts - 1), "twice": _sim_colsum(T, parts, twice=0),
+               "reversed": _sim_colsum(T, parts, order=list(range(parts))[::-1])}
+    if N > 1024:
+        cut = ref.clone()
+        cut[1024:] = 0  # the last 1024-column block never launched
+        defects["last column block"] = cut
+    for name, got in defects.items():
+        with pytest.raises(AssertionError, match="not bit-exact"):
+            R.assert_exact(got, ref, name)  # the fp32 sums (d_gate, d_offset, d_shift are stored unrounded)
+
+
+@pytest.mark.parametrize("M,Rg,budget", [(45, 8, 528), (1003, 100, 256), (700, 1, 256), (1000, 1200, 528)])
+def test_grouped_replay_and_an_unwritten_partial(M, Rg, budget):
+    """The grouped replay equals a row-by-row simulation; a CTA with no rows that leaves its partial unwritten (NaN
+    workspace) changes its group's sum."""
+    g = _gen(M)
+    T = R.rand_bf16((M, 16), g, CPU).float()
+    G, P = -(-M // Rg), R.grouped_parts(M, Rg, budget)
+    acc = torch.zeros(G, P, 16)
+    for row in range(M):
+        gi, r = divmod(row, Rg)
+        acc[gi, r % P] = acc[gi, r % P] + T[row]
+    tot, parts = R.grouped_colsum_replay(T, Rg, budget)
+    assert torch.equal(parts, acc)
+    assert torch.equal(tot, torch.stack([R.partial_sum(acc[i]) for i in range(G)]))
+    last = M - (G - 1) * Rg
+    if last < P:
+        bad = acc.clone()
+        bad[G - 1, P - 1] = float("nan")
+        with pytest.raises(AssertionError):
+            R.assert_exact(R.partial_sum(bad[G - 1]), tot[G - 1], "unwritten partial")
+
+
+def test_row_case_lists_reach_every_path():
+    """The GPU file's case lists reach every launch choice of each entry point."""
+    T = pytest.importorskip("test_gpu_rowops_elementwise")
+    ln = [T.ln_path(M, D, f32, aff, mod, Rg) for M, D, f32, aff, mod, Rg, rl, h in T.LN_CASES]
+    assert {p["warp"] for p in ln} == {True, False}
+    assert {p["nw"] for p in ln if p["warp"]} >= {16, 9, 12, 8}
+    assert {p["stages"] for p in ln if p["warp"]} == {1, 2} and {p["tab_kind"] for p in ln if p["warp"]} == {0, 1, 2}
+    assert any(p["wraps"] > 2 and p["ragged"] for p in ln if p["warp"])
+    assert {p["chunks"] for p in ln if not p["warp"]} == {1, 2, 3, 4}
+    assert any(not p["warp"] and c[2] and c[1] > 6144 for p, c in zip(ln, T.LN_CASES))
+    assert {c[6] for c in T.LN_CASES} == {0, 1, 3} and {c[2] for c in T.LN_CASES} == {True, False}
+    assert {c[5] for c in T.LN_CASES} >= {0, 1} and any(c[5] >= c[0] for c in T.LN_CASES)
+    assert any(c[5] > 1 and c[0] % c[5] for c in T.LN_CASES)
+    assert {c[1] for c in T.LN_CASES} >= {8, 256, 264, 1536, 2048, 2056, 5120, 6144, 8192}
+    rms = [(T.rms_path(M, D, hd, f64), c) for c in T.RMS_CASES for M, D, hd, two, f64, wf, rr, sc in [c]]
+    for warp in (True, False):
+        assert {p["hoisted"] for p, c in rms if p["warp"] == warp} == {True, False}
+        assert any(c[7] for p, c in rms if p["warp"] == warp)  # col_offsets
+        assert any(c[4] for p, c in rms if p["warp"] == warp) and any(c[5] for p, c in rms if p["warp"] == warp)
+    assert {p["stages"] for p, c in rms if p["warp"]} == {1, 2}
+    assert {c[2] for c in T.RMS_CASES} >= {24, 64, 96, 128, 192, 512}
+    assert {c[3] for c in T.SCATTER_CASES} == {"norm", "rope_only", "copy"} and any(c[0] == 1 for c in T.SCATTER_CASES)
+    assert {c[0] for c in T.RMS_BWD_CASES} >= {1, 527, 528, 529, 1063} and {c[0] for c in T.LN_BWD_CASES} >= {1, 527, 528, 529, 1063}
+    assert {T.bwd_path("ln", M, D)["chunks"] for M, D, *_ in T.LN_BWD_CASES} == {1, 2, 3, 4}
+    assert {c[5] for c in T.LN_BWD_CASES} == {None, "bf16", "f32"} and {c[4] for c in T.LN_BWD_CASES} == {0, 1}
+    assert {c[3] for c in T.LN_BWD_CASES} == {True, False} and {c[2] for c in T.LN_BWD_CASES} == {True, False}
+    bias = [T.bwd_path("bias", M, N) for M in T.BIAS_M for N in T.BIAS_N]
+    assert {p["col_blocks"] for p in bias} == {1, 2, 5} and {p["unrolled"] for p in bias} == {True, False}
+    for kind, budget in (("ln_grouped", R.RB_CTAS), ("gate_grouped", R.BG_PARTS)):
+        gp = [(T.bwd_path(kind, M, N, Rg), Rg) for M, Rg, N in T.GROUPED_CASES]
+        assert any(p["G"] == 1 and p["P"] == min(budget, Rg) for p, Rg in gp)
+        assert any(p["G"] > budget and p["P"] == 1 for p, Rg in gp)
+        assert any(p["P"] == Rg and p["G"] > 1 for p, Rg in gp)
+        assert any(p["last"] < Rg and p["empty_parts"] for p, Rg in gp)
+        assert any(p["G"] == 21 and Rg == 1560 for p, Rg in gp)
