@@ -607,3 +607,187 @@ def test_row_case_lists_reach_every_path():
         assert any(p["P"] == Rg and p["G"] > 1 for p, Rg in gp)
         assert any(p["last"] < Rg and p["empty_parts"] for p, Rg in gp)
         assert any(p["G"] == 21 and Rg == 1560 for p, Rg in gp)
+
+
+# ------------------------------------------------------------------------------------------------ convolutions
+def _conv_operands(g, T_in, H, W, Cin, Cout, k, pad=0):
+    x = R.grid_bf16((T_in, H, W, Cin), g, CPU).float()
+    w = R.grid_bf16((Cout, k[0] * k[1] * k[2], Cin + pad), g, CPU).float()
+    return x, w
+
+
+@pytest.mark.parametrize("k,t_off,T_out", [((3, 3, 3), 0, 3), ((3, 3, 3), 1, 2), ((3, 3, 3), 2, 1), ((1, 1, 1), 0, 2),
+                                           ((1, 3, 3), 0, 2), ((3, 1, 1), 1, 2)])
+def test_conv_reference_matches_torch_conv3d(k, t_off, T_out):
+    """conv_exact against F.conv3d (fp32, grid operands: exact) on the causal, zero-padded input, channels past Cin
+    ignored, frames past t_off + T_out unused."""
+    import torch.nn.functional as F
+    g = _gen(1)
+    T_in, H, W, Cin, Cout = t_off + T_out + 1, 9, 17, 24, 40
+    x, w = _conv_operands(g, T_in, H, W, Cin, Cout, k, pad=8)
+    x[t_off + T_out:] = 1e30
+    e, A = R.conv_exact(x, w, k, T_out, t_off)
+    kt, kh, kw = k
+    xc = x[:t_off + T_out].permute(3, 0, 1, 2)[None]
+    xc = F.pad(xc, (kw // 2, kw // 2, kh // 2, kh // 2, kt - 1, 0))
+    wc = w[:, :, :Cin].reshape(Cout, kt, kh, kw, Cin).permute(0, 4, 1, 2, 3)
+    ref = F.conv3d(xc, wc)[0, :, -T_out:].permute(1, 2, 3, 0)
+    assert torch.equal(e.float(), ref)
+    assert bool((A >= e.abs()).all())
+    R.assert_conv_exact_premise(A, 2.0 ** -8, "grid")
+
+
+def test_conv_reference_matches_fp8_restatement():
+    """conv_exact on e4m3 operands against vae_fp8_ref.fp8_conv3d_exact (channels-first, F.conv3d in fp64)."""
+    import vae_fp8_ref
+    g = _gen(2)
+    x = torch.randn(4, 8, 16, 32, generator=g).clamp(-400, 400).to(torch.float8_e4m3fn)
+    w = (torch.randn(48, 32, 3, 3, 3, generator=g) * 4).to(torch.float8_e4m3fn)
+    ws = torch.rand(48, generator=g) + 0.5
+    y = vae_fp8_ref.fp8_conv3d_exact(x.float().permute(3, 0, 1, 2)[None], 0.25, w.float(), ws)[0].permute(1, 2, 3, 0)
+    e, _ = R.conv_exact(x.float(), w.float().permute(0, 2, 3, 4, 1).reshape(48, 27, 32), (3, 3, 3), 4, 0)
+    assert torch.allclose(e * 0.25 * ws.double(), y, rtol=1e-12, atol=1e-9)
+
+
+def test_conv_probe_weights_cover_every_tap_and_chunk():
+    g = _gen(3)
+    for Cout, ntaps, Cin in ((96, 27, 96), (192, 27, 384), (104, 9, 48), (128, 3, 128)):
+        w = R.probe_weights(Cout, ntaps, Cin, Cin + 32, g, CPU)
+        nz = (w != 0).sum((1, 2))
+        assert bool((nz >= 1).all() and (nz <= 3).all()) and bool((w[:, :, Cin:] == 0).all())
+        taps, chunks = R.probe_coverage(Cout, ntaps, Cin)
+        assert taps == set(range(ntaps)) and chunks == set(range(-(-Cin // 32)))
+        single = w[0::3]
+        assert bool(((single != 0).sum((1, 2)) == 1).all())
+        for j in range(single.shape[0]):
+            tap, ch = (single[j] != 0).nonzero()[0].tolist()
+            assert tap == j % ntaps and ch // 32 == j % -(-Cin // 32)
+
+
+def test_conv_case_lists_reach_every_instantiation():
+    """The GPU file's dispatch cases reach every (fp8, BN, BK, NORM, KSUB) the host can launch, with the channel counts
+    whose TMA box runs past Cin, every Cout boundary, every spatial and time edge."""
+    T = pytest.importorskip("test_gpu_conv_elementwise")
+    cases = T.DISPATCH_CASES + T.EDGE_CASES + T.NORM_CASES + T.PERSISTENT_CASES
+    reached = {T.conv_path(c["Cin"], c["Cout"], c["fp8"], c["norm"]) for c in cases}
+    assert reached == T.conv_instantiations() and len(reached) == 77
+    # the host's tile choice, restated: BN by Cout boundaries, BK by Cin_pad, KSUB where three k-blocks share a stage
+    assert [T.conv_path(64, n, False, 0)[1] for n in (16, 17, 96, 97, 128, 129)] == [16, 96, 96, 128, 128, 192]
+    assert {c["Cin"] for c in cases if not c["fp8"]} >= {16, 40, 72} and 48 in {c["Cin"] for c in cases if c["fp8"]}
+    assert {c["W"] for c in cases} >= {1, 15, 16, 17, 33} and {c["H"] for c in cases} >= {1, 7, 8, 9}
+    assert {(c["k"][0], c["t_off"]) for c in cases} >= {(3, 0), (3, 1), (3, 2), (1, 0)}
+    assert max(c["T_out"] for c in cases if c["k"][0] == 3) == 4
+    assert {c["interleave"] for c in cases} >= {32, 64, 384}
+    assert {c["Cout"] for c in cases} >= {3, 200, 384, 576, 768}
+    assert any(c["fp8"] and c["Cout"] > 512 for c in cases)
+    assert any(c["out_gap"] % 2 for c in cases) and any(c["out_off"] % 2 for c in cases)
+    assert any(c["resid"] and c["resid_gap"] for c in cases)
+    norm = [c for c in cases if c["norm"]]
+    assert {c["Cout"] for c in norm} >= {24, 96, 128, 136, 192}
+    assert {(c["fp8"], c["norm"], c["raw"], c["silu"]) for c in norm} >= {(f, n, r, False) for f in (0, 1) for n in (1, 2)
+                                                                         for r in (0, 1)}
+    assert any(c["bound0"] for c in norm) and any(c["norm_gap"] for c in norm)
+
+
+def _norm_row(g, P, C):
+    return R.rand_bf16((P, C), g, CPU)
+
+
+def test_conv_norm_replay_matches_the_formula():
+    """The fused norm's replay and the row pass's replay against the fp64 formula (a few fp32 ulp apart), their sums of
+    squares against an fp64 sum, and the e4m3 code against vae_fp8_ref.quantize_static where v is not -0."""
+    import vae_fp8_ref
+    g = _gen(4)
+    for C in (24, 96, 136, 192, 8, 264, 384):
+        y = _norm_row(g, 300, C)
+        y[0] = 0  # the 1e-12 floor
+        gamma = 1 + 0.2 * torch.randn(C, generator=g)
+        y64 = y.double()
+        ref = y64 / y64.norm(dim=1, keepdim=True).clamp_min(1e-12) * math.sqrt(C) * gamma.double()
+        for v in ([R.conv_norm_replay(y, gamma, C)] if C <= 192 else []) + [R.rownorm_replay(y, gamma)]:
+            assert torch.allclose(v.double(), ref, rtol=2 ** -20, atol=1e-30)
+        ss = R.norm_sum_replay(y, C) if C <= 192 else None
+        if ss is not None:
+            assert torch.allclose(ss.double(), (y.double() ** 2).sum(1), rtol=C * 2 ** -24)
+        bound = vae_fp8_ref.norm_bound(gamma)
+        v = R.rownorm_replay(y, gamma)
+        code = R.e4m3_code(v, R.e4m3_qscale(bound))
+        pos = v != 0
+        assert torch.equal(code.view(torch.uint8)[pos], vae_fp8_ref.quantize_static(v, bound).view(torch.uint8)[pos])
+    assert R.e4m3_code(torch.tensor([-1.0, 1.0]), 0.0).view(torch.uint8).tolist() == [0x80, 0]
+
+
+def test_conv_norm_checkers_reject_defects():
+    """A norm with sqrt(BN) in place of sqrt(Cout), a sum that skips the last column group, and one e4m3 code a step off
+    fail the exact check; SiLU outputs one bf16 ulp off the interval fail assert_rounds_from."""
+    g = _gen(5)
+    C = 104
+    y = _norm_row(g, 500, C)
+    gamma = 1 + 0.2 * torch.randn(C, generator=g)
+    qs = R.e4m3_qscale(math.sqrt(C) * float(gamma.abs().max()))
+    good = R.e4m3_code(R.conv_norm_replay(y, gamma, C), qs).view(torch.uint8)
+    bad_bn = R.e4m3_code(R.conv_norm_replay(y, gamma, C, sqrt_of=128), qs).view(torch.uint8)
+    with pytest.raises(AssertionError):
+        R.assert_exact(bad_bn, good, "sqrt(BN)")
+    short = R.e4m3_code(R.conv_norm_replay(y[:, :96].contiguous(), gamma[:96], 96, sqrt_of=C), qs).view(torch.uint8)
+    with pytest.raises(AssertionError):
+        R.assert_exact(short, good[:, :96], "a column group missing from the sum")
+    step = good.clone()
+    step[7, 11] += 1
+    with pytest.raises(AssertionError):
+        R.assert_exact(step, good, "one code one step off")
+    v = R.conv_norm_replay(y, gamma, C)
+    ref, b = R.silu_bound(v)
+    got = (v.double() * torch.sigmoid(v.double())).float().bfloat16()
+    assert R.assert_rounds_from(got.float(), ref, b, "silu") < 0.05
+    off = got.float().clone()
+    off[3, 4] = torch.nextafter(off[3, 4].bfloat16(), torch.tensor(1e30, dtype=torch.bfloat16)).float()
+    off[3, 4] = off[3, 4] + R.ulp_bf16(off[3, 4:5]).float()[0]
+    with pytest.raises(AssertionError):
+        R.assert_rounds_from(off, ref, b, "one ulp off")
+
+
+def test_conv_checkers_reject_data_movement_defects():
+    """On a CPU-simulated grid output: one tap dropped in a border tile, one tile's halo shifted by a pixel, two 8-column
+    groups swapped in the second N block, bias column n - 512 for n >= 512, interleave frames swapped."""
+    g = _gen(6)
+    k, T_out, t_off = (3, 3, 3), 2, 1
+    x, w = _conv_operands(g, 4, 9, 33, 16, 600, k)
+    bias = R.grid_bf16((600,), g, CPU)
+    e, A = R.conv_exact(x, w, k, T_out, t_off)
+    R.assert_conv_exact_premise(A, 2.0 ** -8, "sim")
+    ref = R.conv_epilogue_ref(e.float(), bias)
+    where = lambda i: R.conv_coords(i, 192)
+
+    def rejected(m, name):
+        with pytest.raises(AssertionError):
+            R.assert_exact(m, ref, name, where)
+
+    w2 = w.clone()
+    w2[:, 18] = 0  # tap (dt 2, dh 0, dw 0): pixel (8, 32) reads (7, 31) through it
+    m = ref.clone()
+    m[:, 8:, 32:] = R.conv_epilogue_ref(R.conv_exact(x, w2, k, T_out, t_off, False)[0].float(), bias)[:, 8:, 32:]
+    rejected(m, "tap dropped")
+    m = ref.clone()
+    m[:, :8, 16:32] = R.conv_epilogue_ref(R.conv_exact(torch.roll(x, 1, 2), w, k, T_out, t_off, False)[0].float(),
+                                          bias)[:, :8, 16:32]
+    rejected(m, "halo shifted")
+    m = ref.clone()
+    m[..., 192:200], m[..., 200:208] = ref[..., 200:208], ref[..., 192:200]
+    rejected(m, "column groups swapped")
+    rejected(R.conv_epilogue_ref(e.float(), torch.cat([bias[:512], bias[:88]])), "bias n - 512")
+    il = torch.stack([ref[..., :300], ref[..., 300:]], 1).flatten(0, 1)  # frames 2t, 2t + 1
+    swapped = torch.stack([ref[..., 300:], ref[..., :300]], 1).flatten(0, 1)
+    assert not torch.equal(il, swapped)
+    assert R.conv_coords((1, 8, 32, 200), 192) == dict(t=1, y=8, x=32, n=200, tile=(1, 2), row=0, warpgroup=0, warp=0,
+                                                        n_blk=1, col_group=1)
+
+
+def test_softmax_bound_holds_for_float32_softmax():
+    g = _gen(7)
+    x = torch.randn(6, 1350, generator=g) * 4
+    x[2, ::7] = float("-inf")
+    ref, b = R.softmax_bound(x)
+    got = torch.softmax(x, -1).bfloat16()
+    R.assert_within(got, ref, b, "torch fp32 softmax")
+    assert bool(((b / ref.clamp_min(1e-300))[ref > 1e-30] < 2 ** -7).all())
